@@ -1,8 +1,8 @@
 #!/usr/bin/env python
-"""bench.py -- Groth16 proofs/s on the co-snarks hot path (BASELINE.json metric), B200.
+"""bench.py -- Groth16 proofs/s on the co-snarks hot path (BASELINE.json metric), H100.
 
 A "step" = one Groth16 proof over BN254 for a synthetic 2^20-constraint R1CS (BASELINE.json
-configs[1]: plain prover, 1xB200): witness map (2 SpMV, 6 NTT of 2^20, 3 element kernels) + 5 MSMs
+configs[1]: plain prover, 1xH100): witness map (2 SpMV, 6 NTT of 2^20, 3 element kernels) + 5 MSMs
 (4 G1 + 1 G2 of ~2^20) + assembly, through the reference-facing C ABI (cs_groth16_prove_plain).
   value : proofs/s with the witness already resident in HBM (cs_groth16_prove_plain_device), CUDA events
   e2e   : the same through host (pinned) buffers -- H2D of the witness and D2H of the results inside
@@ -10,6 +10,9 @@ configs[1]: plain prover, 1xB200): witness map (2 SpMV, 6 NTT of 2^20, 3 element
   N > 1 : N independent prover replicas, one per GPU (the path shards by proof; no data-path
           collective), barrier + max over ranks, value = N*K / t      ("scaling": "weak")
   --impl reference : the oracle's C restatement of the reference CPU path (oracle/c) on the host cores.
+  --dump-outputs DIR : after the timed steps, rank 0 writes the proof (A, B, C) of the last timed step as
+          DIR/proof_{a,b,c}.npy: the affine Montgomery limbs the C ABI returns, as 32-bit words in float64 (exact).
+          Inputs are seeded, so two builds run with the same arguments can be compared output for output.
 Prints ONE JSON line on rank 0.
 
 oracle/ is used here only as the checker and the CPU baseline, never inside a timed region and never by the
@@ -35,11 +38,7 @@ METRIC = "co-Groth16 proofs/sec (BN254, 2^20 constraints); MSM Mscalar/s"
 
 
 def peaks():
-    p = os.path.join(ROOT, "MEASURED_PEAKS.json")
-    if os.path.exists(p):
-        j = json.load(open(p))
-        return float(j["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs, burst copy)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet (HBM3), not measured"
 
 
 class ClockSampler:
@@ -181,7 +180,7 @@ def rep3_threads_one_gpu(args, ctx, pk, syn):
     ms_dev, _ = run(args.steps, True)
     sent = (nets0[0].bytes_sent + nets1[0].bytes_sent - sent0) // args.steps
     ms_host, _ = run(args.steps, False)
-    out = {"layout": "3 parties as 3 host threads sharing 1xB200 (one context, key and stream set per party)",
+    out = {"layout": "3 parties as 3 host threads sharing 1xH100 (one context, key and stream set per party)",
            "gpus": 1, "groups": 1, "gpus_per_party": "1/3",
            "ms_per_proof": ms_dev / args.steps, "proofs_per_s": args.steps / (ms_dev * 1e-3),
            "e2e_ms_per_proof": ms_host / args.steps, "e2e_proofs_per_s": args.steps / (ms_host * 1e-3),
@@ -218,7 +217,7 @@ def plonk_rep3_block(args, rank, local_rank):
     if res is None:
         return None
     r = res["2p%d" % lg]
-    return {"workload": "co-Plonk Rep3, BN254, synthetic snarkjs-style circuit, domain 2^%d, 3 parties on 3xB200 "
+    return {"workload": "co-Plonk Rep3, BN254, synthetic snarkjs-style circuit, domain 2^%d, 3 parties on 3xH100 "
                         "(BASELINE.json configs[3])" % lg,
             "ms_per_proof": r["ms_per_proof"], "proofs_per_s": r["proofs_per_s"], "pairing_verified": r["verified"],
             "net_bytes_per_party_per_proof": r["bytes_sent_per_party"], "key_setup_s": r["setup_s"],
@@ -428,7 +427,7 @@ def run_ours(args):
         e0.record(stream)
         tw0 = time.perf_counter()
         for _ in range(args.steps):
-            pk.prove_plain_device(pub, d_wit, r_m, s_m)
+            last_proof = pk.prove_plain_device(pub, d_wit, r_m, s_m)
         e1.record(stream)
     torch.cuda.synchronize()
     tw1 = time.perf_counter()
@@ -437,6 +436,8 @@ def run_ours(args):
     value_ms = max_over_ranks(max(dev_ms, (tw1 - tw0) * 1e3))
     launches = ctx.launch_count() - l0
     barrier()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last_proof)
 
     timeline = None
     if args.timeline and rank == 0:
@@ -541,7 +542,7 @@ def run_ours(args):
         ntt_avg = sum(ntt_ms) / len(ntt_ms)
         ctx.free(d_v)
         dom.free()
-        gmul_peak, imad_tops, peak_src = int_pipe_ceiling()
+        gmul_peak, peak_src = int_pipe_ceiling()
         g1_madds = 16.0 * nw  # W = 16 windows: one mixed addition (8M + 2S = 10 products) per scalar per window
         gmul = g1_madds * 10 / (accum_ms * 1e-3) / 1e9
         steps_total = args.steps * world
@@ -550,10 +551,10 @@ def run_ours(args):
             "steps": args.steps, "warmup": args.warmup, "ms_per_step": value_ms / args.steps,
             "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "u32x8 (256-bit Montgomery, integer)",
             "data": "synthetic (seeded R1CS + known-toxic-waste key; proof pairing-verified: %s)" % proof_ok,
-            "config": {"workload": "plain Groth16 prover, BN254, synthetic R1CS 2^%d constraints, 1xB200 per replica "
+            "config": {"workload": "plain Groth16 prover, BN254, synthetic R1CS 2^%d constraints, 1xH100 per replica "
                                    "(BASELINE.json configs[1])" % lg,
                        "domain": n, "window_bits": pk_window(args, n), "replicas": world,
-                       "l2": "working set (5 precomputed base tables, ~6.4 GB) exceeds the 126 MB L2; no flush needed",
+                       "l2": "working set (5 precomputed base tables, ~6.4 GB) exceeds the 50 MB L2; no flush needed",
                        "setup_s": round(setup_s, 1), "key_upload_s": round(key_upload_s, 2),
                        "time_to_first_proof_note": "key_upload_s = cs_groth16_pk_create alone (CSR + 5 query arrays uploaded and "
                                                    "expanded to per-window tables); setup_s adds the synthesis of the synthetic key"},
@@ -563,15 +564,11 @@ def run_ours(args):
             "gpu_launches": int(launches),
             "clocks": clk,
             "roofline": {"kernel": "k_msm_accum0<Fp<Bn254Fq>> (G1 bucket accumulation)", "bound": "hbm",
-                         "achieved": achieved, "peak": hbm, "unit": "GB/s", "frac": achieved / hbm,
-                         "traffic": ncu_traffic(), "peak_source": hbm_src,
-                         "traffic_source": "profiles/r2_ncu_full_accum0_g1.csv (ncu --set full of this kernel on a dense 2^20 G1 MSM; "
-                                           "bytes per launch). 16 precomputed table points are read per scalar by design (no doublings), "
-                                           "HBM stays below 10 % busy",
+                         "achieved": achieved, "peak": hbm, "unit": "GB/s", "frac": achieved / hbm, "peak_source": hbm_src,
                          "note": "256-bit modular arithmetic is integer-pipe bound (~2.3 kIMAD per 96 B); see DESIGN.md",
                          "launch_ms": accum_ms, "algorithmic_bytes_per_launch": alg_bytes,
                          "int_pipe": {"achieved_gmodmul_s": gmul, "peak_gmodmul_s": gmul_peak, "frac": gmul / gmul_peak,
-                                      "imad_wide_tops": imad_tops, "imad_wide_tops_source": "profiles/r2_pipe_probe.json (data-dependent operands)", "peak_source": peak_src,
+                                      "peak_source": peak_src,
                                       "note": "the resource that actually bounds the kernel: 10 Montgomery products per mixed addition, counted as 10 although two of them (R (Q - X3) - Y1 PPP) share one reduction (Fp::dot2, 1.5 product-equivalents of multiply work)"}},
             "msm": {"g1_2p%d_ms" % lg: msm_avg, "mscalar_per_s": nw / (msm_avg * 1e-3) / 1e6,
                     "stage_ms": {"digits": float(stage[0]), "sort": float(stage[1]), "accumulate": float(stage[2]),
@@ -597,19 +594,13 @@ def run_ours(args):
         print(json.dumps(out))
 
 
-def ncu_traffic():
-    """dram__bytes_read.sum + dram__bytes_write.sum of the accumulate kernel from the committed ncu summary."""
-    path = os.path.join(ROOT, "profiles", "r2_ncu_full_accum0_g1.csv")
-    mult = {"byte": 1.0, "Kbyte": 1e3, "Mbyte": 1e6, "Gbyte": 1e9}
-    try:
-        tot = 0.0
-        for line in open(path):
-            f = line.strip().split(",")
-            if f[0] == "0" and f[1] in ("dram__bytes_read.sum", "dram__bytes_write.sum"):
-                tot += float(f[3].strip('"')) * mult[f[2]]
-        return tot or None
-    except OSError:
-        return None
+def dump_outputs(out_dir, proof):
+    """The proof (A, B, C) as the C ABI returns it: affine Montgomery u64 limbs, written as their 32-bit halves in
+    float64 so that every bit survives the float format."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    for name, arr in zip(("proof_a", "proof_b", "proof_c"), proof):
+        np.save(os.path.join(out_dir, name + ".npy"), np.ascontiguousarray(arr, dtype=np.uint64).view(np.uint32).astype(np.float64))
 
 
 def run_rep3(args):
@@ -673,7 +664,7 @@ def run_plonk_rep3(args):
         "n_gpus": 3, "steps": args.steps, "warmup": 1, "ms_per_step": r["ms_per_proof"], "higher_is_better": True,
         "scaling": "weak", "vs_baseline": None, "dtype": "u32x8 (256-bit Montgomery, integer)",
         "data": "synthetic snarkjs-style Plonk circuit with a valid key; proof accepted by the oracle's verifier: %s" % r["verified"],
-        "config": {"workload": "co-Plonk Rep3, BN254, synthetic circuit domain size 2^%d, 3 parties on 3xB200 "
+        "config": {"workload": "co-Plonk Rep3, BN254, synthetic circuit domain size 2^%d, 3 parties on 3xH100 "
                                "(BASELINE.json configs[3])" % args.log_m, "setup_s": r["setup_s"]},
         "e2e": {"value": r["proofs_per_s"], "unit": "proofs/s", "note": "host share buffers in, opened proof out, wall clock, max over ranks"},
         "net_bytes_per_party_per_proof": r["bytes_sent_per_party"]}))
@@ -681,17 +672,11 @@ def run_plonk_rep3(args):
 
 def int_pipe_ceiling():
     """Measured ceiling of 256-bit Montgomery products on the integer pipe (tools/imad_peak, built by
-    __graft_entry__.build()); falls back to the committed measurement of this pool's B200."""
+    __graft_entry__.build()), measured live on the GPU the bench runs on."""
     exe = os.path.join(ROOT, "tools", "imad_peak")
-    try:
-        out = subprocess.run([exe], capture_output=True, text=True, timeout=120).stdout
-        j = json.loads(out)
-        # the probe's own "imad_wide_tops" loop has loop-invariant operands that ptxas strength-reduces to adds (it reads
-        # 17 T/s); the IMAD.WIDE issue rate with data-dependent operands is 9.2 T/s (tools/pipe_probe.cu,
-        # profiles/r2_pipe_probe.json), which is what the Montgomery ceiling below reflects
-        return max(v for k, v in j.items() if k.startswith("montmul_gmuls")), 9.2, "measured live (tools/imad_peak)"
-    except Exception:  # noqa: BLE001
-        return 65.2, 9.2, "committed measurement (profiles/r1_imad_peak_and_multiplier_variants.json)"
+    out = subprocess.run([exe], capture_output=True, text=True, timeout=120, check=True).stdout
+    j = json.loads(out)
+    return max(v for k, v in j.items() if k.startswith("montmul_gmuls")), "measured live (tools/imad_peak)"
 
 
 def pk_window(args, n):
@@ -736,6 +721,8 @@ def main():
     ap.add_argument("--timeline", action="store_true",
                     help="after the timed region: one more proof with stage events, reported as timeline_ms (diagnostic)")
     ap.add_argument("--no-cpu-baseline", action="store_true", help="diagnostic runs: skip the CPU leg")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the proof of the last timed step as DIR/proof_{a,b,c}.npy (plain mode, rank 0)")
     args = ap.parse_args()
     if args.warmup < 3:
         args.warmup = 3

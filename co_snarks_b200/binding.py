@@ -227,7 +227,7 @@ _LIBS = {}
 
 def load(path=None, strict=True):
     """Load the shared library and attach signatures.  Raises if it is missing -- build it with
-    `python -c "import __graft_entry__ as g; g.build()"` (nvcc, sm_100a)."""
+    `python -c "import __graft_entry__ as g; g.build()"` (nvcc, sm_90a)."""
     path = os.path.abspath(path or DEFAULT_LIB)
     if path in _LIBS:
         return _LIBS[path]

@@ -1,4 +1,4 @@
-"""nvcc build of libcosnarks_gpu.so for sm_100a (in-tree, so the .so travels with gpurun snapshots)."""
+"""nvcc build of libcosnarks_gpu.so for sm_90a (H100), in-tree next to the package."""
 import os
 import subprocess
 import sys
@@ -7,7 +7,8 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 OUT = os.path.join(HERE, "libcosnarks_gpu.so")
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+GENCODE = ["-gencode", "arch=compute_90a,code=sm_90a"]
+FLAGS = GENCODE + ["-lineinfo", "-O3", "-std=c++17",
          "--expt-relaxed-constexpr", "-DCS_ENABLE_BLS12_381", "-Xcompiler", "-fPIC", "-Xcompiler", "-O2", "-shared", "-cudart", "static"]
 
 
@@ -41,7 +42,7 @@ def build(force=False, verbose=False, extra=()):
             sys.stdout.write(out)
         if p.returncode:
             raise RuntimeError("nvcc failed: " + " ".join(cmd))
-    subprocess.check_call([NVCC, "-shared", "-cudart", "static", "-gencode", "arch=compute_100a,code=sm_100a", "-o", OUT] + objs)
+    subprocess.check_call([NVCC, "-shared", "-cudart", "static"] + GENCODE + ["-o", OUT] + objs)
     return OUT
 
 

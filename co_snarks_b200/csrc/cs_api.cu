@@ -21,8 +21,7 @@ int fail(int code, const char* fmt, ...) {
 #if !defined(CS_EMU)
 // The prover keeps up to 12 streams busy at once (five MSMs x {sort/fold/reduce, accumulation}, witness map, caller's
 // stream).  The driver multiplexes streams onto CUDA_DEVICE_MAX_CONNECTIONS hardware queues (default 8); streams that
-// share a queue serialise -- measured: the L MSM did not start until the H MSM, 14 ms of unrelated work, had drained
-// (profiles/r2_prio_ab2.log).  The variable is read when the CUDA context is created, so it is set when this library is
+// share a queue serialise (the L MSM would not start until the unrelated H MSM had drained).  The variable is read when the CUDA context is created, so it is set when this library is
 // loaded, unless the application chose a value itself.
 __attribute__((constructor)) static void cs_more_hw_queues() { setenv("CUDA_DEVICE_MAX_CONNECTIONS", "32", 0); }
 #endif
@@ -72,7 +71,7 @@ const char* cs_version(void) {
 #if defined(CS_EMU)
   return "cosnarks-b200 0.1 (CPU emulation build -- tests only)";
 #else
-  return "cosnarks-b200 0.1 (sm_100a)";
+  return "cosnarks-b200 0.1 (sm_90a)";
 #endif
 }
 
@@ -90,9 +89,8 @@ int cs_ctx_create(int device, void* stream, cs_ctx** out) {
   // Stream priorities (CUDA: lower number = served first).  The short, latency-bound kernels (digit sort, folds,
   // bucket reduction, NTT passes) run on higher-priority streams than the full-GPU MSM accumulation grids, so that
   // they are not queued behind every accumulation launched before them.  CS_PRIO="side,acc,wm" overrides
-  // (default "-2,0,-2"); CS_MSM_SPLIT=0 keeps each MSM on a single stream.  With 32 hardware queues every layout
-  // tried lands within 0.1 ms of the others (17.9-18.0 ms, profiles/r2_sched_ab*.log): the proof is bound by the sum
-  // of its integer-pipe work, the layout only decides which MSM finishes first.
+  // (default "-2,0,-2"); CS_MSM_SPLIT=0 keeps each MSM on a single stream.  The proof is bound by the sum of its
+  // integer-pipe work; the layout only decides which MSM finishes first.
   int prio_side = -2, prio_acc = 0, prio_wm = -2;
   if (const char* e = getenv("CS_PRIO")) sscanf(e, "%d,%d,%d", &prio_side, &prio_acc, &prio_wm);
   const char* split_env = getenv("CS_MSM_SPLIT");
@@ -204,8 +202,8 @@ int bases_upload_t(cs_ctx* ctx, const uint64_t* h_points, size_t n, int window_b
   CS_LAUNCH(k_msm_precompute<F>, ceil_div(n, 128), 128, 0, ctx->stream, b->table.as<Affine<F>>(), (uint32_t)n,
             b->sh.c, b->sh.W);
   // BN254 G1, opt-in (CS_MSM_F52=1): bucket accumulation on the FP64 pipe (cs_msm52.cuh); its table holds the
-  // coordinates in the radix-2^260 Montgomery form.  Measured on B200 (profiles/r2_f52_accum0_ab.log): bit-exact,
-  // 3.06 ms against 2.86 ms for the integer-pipe kernel at 2^20 -- the integer kernel stays the default.
+  // coordinates in the radix-2^260 Montgomery form.  Bit-exact, but the FP64 and integer pipes do not overlap, so
+  // trading IMAD.WIDE for DFMA buys nothing: the integer kernel stays the default.
   if (G == 0 && std::is_same<Cfg, Bn254Cfg>::value) {
     static int f52_env = -1;
     if (f52_env < 0) { const char* e = getenv("CS_MSM_F52"); f52_env = e ? atoi(e) : 0; }
@@ -499,10 +497,9 @@ int ntt_run(cs_ctx* ctx, const cs_domain* d, uint32_t* d_data, unsigned batch, b
             const uint32_t* d_post, cudaStream_t st) {
   if (batch != 1 && batch != 2) return fail(CS_ERR_ARG, "ntt: batch must be 1 or 2");
   if (d->log_n == 0) return 0;
-  // CS_NTT_V2=1 selects the TMA-staged radix-8 pass (cs_ntt8.cuh).  Measured on B200 (profiles/r2_ntt_v1_v2.md): it
-  // ties the round-1 kernel at 2^20 (0.266 vs 0.260 ms, batch 2: 0.4735 vs 0.4743), loses 2-3 % at 2^22 / 2^24 and 2.5x
-  // at 2^16 (tile set-up); both sit at 65 % fmaheavy, the instruction-mix bound of one product + add + sub per
-  // butterfly.  The bulk-copy staging therefore buys nothing here and the default stays the round-1 pass.
+  // CS_NTT_V2=1 selects the TMA-staged radix-8 pass (cs_ntt8.cuh).  Both passes are bound by the instruction mix of a
+  // butterfly (one product + add + sub), not by the copies, and the TMA pass pays a tile set-up at small sizes, so the
+  // bulk-copy staging buys nothing and the default stays the radix-2 pass.
   static int v2_env = -1;
   if (v2_env < 0) { const char* e = getenv("CS_NTT_V2"); v2_env = e ? atoi(e) : 0; }
   CS_DISPATCH_CURVE(d->curve, {
@@ -599,7 +596,7 @@ static int vec_binop(cs_ctx* ctx, cs_curve curve, const uint64_t* a, const uint6
   if (!ctx || !a || !b || !out) return fail(CS_ERR_ARG, "vec op: NULL argument");
   if (n == 0) return 0;
   unsigned blocks = ceil_div(n, 256);
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > CS_NUM_SMS * 16) blocks = CS_NUM_SMS * 16;
   CS_DISPATCH_CURVE(curve, {
     CS_LAUNCH(k_vec_binop<typename Cfg::FrP>, blocks, 256, 0, ctx->stream, reinterpret_cast<const uint32_t*>(a),
               reinterpret_cast<const uint32_t*>(b), reinterpret_cast<uint32_t*>(out), n, op);
@@ -622,7 +619,7 @@ int cs_vec_scale_table(cs_ctx* ctx, cs_curve curve, uint64_t* x, const uint64_t*
   if (batch != 1 && batch != 2) return fail(CS_ERR_ARG, "cs_vec_scale_table: batch must be 1 or 2");
   if (n == 0) return 0;
   unsigned blocks = ceil_div(n * batch, 256);
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > CS_NUM_SMS * 16) blocks = CS_NUM_SMS * 16;
   CS_DISPATCH_CURVE(curve, {
     CS_LAUNCH(k_vec_scale_table<typename Cfg::FrP>, blocks, 256, 0, ctx->stream, reinterpret_cast<uint32_t*>(x),
               reinterpret_cast<const uint32_t*>(table), n, batch);
@@ -636,7 +633,7 @@ int cs_rep3_local_mul_vec(cs_ctx* ctx, cs_curve curve, const uint64_t* a, const 
   if (!ctx || !a || !b || !out) return fail(CS_ERR_ARG, "cs_rep3_local_mul_vec: NULL argument");
   if (n == 0) return 0;
   unsigned blocks = ceil_div(n, 256);
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > CS_NUM_SMS * 16) blocks = CS_NUM_SMS * 16;
   CS_DISPATCH_CURVE(curve, {
     CS_LAUNCH(k_rep3_local_mul<typename Cfg::FrP>, blocks, 256, 0, ctx->stream, reinterpret_cast<const uint32_t*>(a),
               reinterpret_cast<const uint32_t*>(b), reinterpret_cast<const uint32_t*>(mask),
@@ -659,7 +656,7 @@ int cs_vec_lincomb(cs_ctx* ctx, cs_curve curve, const uint64_t* const* d_inputs,
     memcpy(a.w[j], h_weights_mont + 4 * j, 32);
   }
   unsigned blocks = ceil_div(n, 256);
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > CS_NUM_SMS * 16) blocks = CS_NUM_SMS * 16;
   CS_DISPATCH_CURVE(curve, {
     CS_LAUNCH(k_vec_lincomb<typename Cfg::FrP>, blocks, 256, 0, ctx->stream, a, k, reinterpret_cast<uint32_t*>(d_out), n);
   });
@@ -768,7 +765,7 @@ int cs_rep3_batch(cs_ctx* ctx, cs_curve curve, cs_rep3_batch_op op, int party, c
   if (n == 0) return 0;
   CS_CUDA(cudaSetDevice(ctx->device));
   unsigned blocks = ceil_div(n, 256);
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > CS_NUM_SMS * 16) blocks = CS_NUM_SMS * 16;
   CS_DISPATCH_CURVE(curve, {
     CS_LAUNCH(k_rep3_batch<typename Cfg::FrP>, blocks, 256, 0, ctx->stream, (int)op, party, reinterpret_cast<const uint32_t*>(d_x),
               reinterpret_cast<const uint32_t*>(d_y), reinterpret_cast<uint32_t*>(d_out), n);
@@ -782,7 +779,7 @@ int cs_rep3_batch_open_send(cs_ctx* ctx, cs_curve curve, const uint64_t* d_share
   if (n == 0) return 0;
   CS_CUDA(cudaSetDevice(ctx->device));
   unsigned blocks = ceil_div(n, 256);
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > CS_NUM_SMS * 16) blocks = CS_NUM_SMS * 16;
   CS_DISPATCH_CURVE(curve, {
     CS_LAUNCH(k_rep3_take_b<typename Cfg::FrP>, blocks, 256, 0, ctx->stream, reinterpret_cast<const uint32_t*>(d_shares),
               reinterpret_cast<uint32_t*>(d_next_recv), n);
@@ -797,7 +794,7 @@ int cs_rep3_batch_open_finish(cs_ctx* ctx, cs_curve curve, const uint64_t* d_sha
   if (n == 0) return 0;
   CS_CUDA(cudaSetDevice(ctx->device));
   unsigned blocks = ceil_div(n, 256);
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > CS_NUM_SMS * 16) blocks = CS_NUM_SMS * 16;
   CS_DISPATCH_CURVE(curve, {
     CS_LAUNCH(k_rep3_batch<typename Cfg::FrP>, blocks, 256, 0, ctx->stream, (int)R3B_OPEN_FINISH, 0,
               reinterpret_cast<const uint32_t*>(d_shares), reinterpret_cast<const uint32_t*>(d_recv),
@@ -888,7 +885,7 @@ int cs_rep3_to_shamir(cs_ctx* ctx, cs_curve curve, const uint64_t* x, const uint
   CS_CUDA(cudaMemcpyAsync(ctx->io.p, h_ca, 32, cudaMemcpyHostToDevice, ctx->stream));
   CS_CUDA(cudaMemcpyAsync((char*)ctx->io.p + 32, h_cb, 32, cudaMemcpyHostToDevice, ctx->stream));
   unsigned blocks = ceil_div(n, 256);
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > CS_NUM_SMS * 16) blocks = CS_NUM_SMS * 16;
   CS_DISPATCH_CURVE(curve, {
     CS_LAUNCH(k_rep3_to_shamir<typename Cfg::FrP>, blocks, 256, 0, ctx->stream, reinterpret_cast<const uint32_t*>(x),
               ctx->io.as<uint32_t>(), ctx->io.as<uint32_t>() + 8, reinterpret_cast<uint32_t*>(out), n);

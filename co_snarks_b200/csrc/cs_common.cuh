@@ -23,6 +23,9 @@
 
 #define COMMA ,
 
+// SMs of an H100 SXM; grid-stride kernels cap their grids at a small multiple of it.
+#define CS_NUM_SMS 132
+
 // NVTX ranges named after the reference's `tracing` spans (co-groth16/src/groth16.rs:230-313,
 // groth16/reduction.rs:98-184), so an nsys / ncu --nvtx timeline of a proof reads like the reference's
 // trace output.  No-ops in the emulation build; near-free when no tool is attached.

@@ -1,9 +1,8 @@
 // Prime-field multiplication on the FP64 pipe: 5 limbs of 52 bits, Montgomery radix R = 2^260.
 //
-// Why: measured on B200 (profiles/r2_pipe_probe.json, tools/pipe_probe.cu) IMAD.WIDE.U32 -- the instruction the
-// 8 x 32-bit CIOS product is made of -- issues at HALF the IMAD rate (9.2 T/s, 4 cycles per warp instruction per
-// SM sub-partition; round 1's "17.3 T/s" was ptxas strength-reducing the probe to IADD3), while DFMA issues at
-// the full rate (18.3 T/s, 2 cycles).  A 52 x 52 -> 104-bit limb product costs two DFMA + one DADD (6 pipe
+// Why: IMAD.WIDE.U32 -- the instruction the 8 x 32-bit CIOS product is made of -- issues at HALF the IMAD rate
+// (4 cycles per warp instruction per SM sub-partition), while DFMA issues at the full rate (2 cycles);
+// tools/pipe_probe.cu measures both.  A 52 x 52 -> 104-bit limb product costs two DFMA + one DADD (6 pipe
 // cycles for 2704 bit^2) against 4 cycles per 1024 bit^2 for IMAD.WIDE: the same modular product needs
 // ~170 FP64-pipe instructions (340 cycles) instead of ~150 IMAD-pipe instructions (600 cycles).
 //

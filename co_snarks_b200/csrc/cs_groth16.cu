@@ -117,7 +117,7 @@ int witness_map_device(cs_ctx* ctx, cs_groth16_pk* pk, int kind, int party, cons
             pub_comp, (uint32_t)pk->nc, 0u, n, pk->d_b.as<uint32_t>());
   }
   unsigned blocks = ceil_div(n, 256);
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > CS_NUM_SMS * 16) blocks = CS_NUM_SMS * 16;
   // c = local_mul_vec(a, b)   (reduction.rs:160)
   CS_SPAN("c: local_mul_vec / a, b, c: distribute powers (fft/ifft)");
   if (kind == CS_REP3)
@@ -219,7 +219,7 @@ int witness_map_libsnark_device(cs_ctx* ctx, cs_groth16_pk* pk, int kind, int pa
   CS_TRY(ntt_run(ctx, pk->dom_ark, pk->d_c.as<uint32_t>(), 1, true, post, st));
   CS_TRY(ntt_run(ctx, pk->dom_ark, pk->d_c.as<uint32_t>(), 1, false, nullptr, st));
   unsigned blocks = ceil_div(n, 256);
-  if (blocks > 148 * 16) blocks = 148 * 16;
+  if (blocks > CS_NUM_SMS * 16) blocks = CS_NUM_SMS * 16;
   // ab = local_mul_vec(a, b) - c   (reduction.rs:289, :316-322; the constant factor is folded into the iNTT below)
   if (kind == CS_REP3)
     CS_LAUNCH(k_rep3_local_mul<FrP>, blocks, 256, 0, st, pk->d_a.as<uint32_t>(), pk->d_b.as<uint32_t>(),
@@ -272,8 +272,8 @@ int local_phase(cs_ctx* ctx, cs_groth16_pk* pk, int kind, int party, const uint6
   CS_TRY(upload_inputs(ctx, pk, kind, h_pub, h_wit, do_h ? h_m1 : nullptr, do_h ? h_m2 : nullptr));
   // fork: A, B1, B2, L need only the witness.  The witness map -> H chain is the longest dependency chain of the proof
   // (6-10 NTTs, then a full MSM), so it is enqueued FIRST and on the highest-priority stream: its passes interleave
-  // with the other MSMs' accumulation grids instead of queueing behind all of them (profiles/r2_prio_ab.log: before,
-  // H started 14.8 ms into an 18.9 ms proof, after the four side MSMs had drained).
+  // with the other MSMs' accumulation grids instead of queueing behind all of them (otherwise H starts only after the
+  // four side MSMs have drained).
   CS_TRY(ctx_fork(ctx, 4));
   cudaStream_t wm = ctx->wm;
   CS_CUDA(cudaStreamWaitEvent(wm, ctx->ev_fork, 0));

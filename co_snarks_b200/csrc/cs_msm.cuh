@@ -1,12 +1,12 @@
-// Multi-scalar multiplication  sum_i s_i * P_i  on sm_100a.
+// Multi-scalar multiplication  sum_i s_i * P_i  on sm_90a.
 //
 // Replaces `taceo_ark_algebra::msm::{msm_unchecked, msm_bigint}` (taceo-ark-algebra 0.1.0, not
 // vendored; call sites co-groth16/src/mpc/{plain.rs:66-74, rep3.rs:124-132, shamir.rs:111-119},
 // co-groth16/src/groth16.rs:190-200, mpc-core/src/protocols/rep3/pointshare.rs:201-222).
 //
-// B200-first design (DESIGN.md "MSM"):
+// Design (DESIGN.md "MSM"):
 //  * The base set is a proving key / SRS: it is uploaded once and expanded to a table of
-//    2^(c w) * P_i for every window w (180 GB of HBM makes W x the key size affordable).  All
+//    2^(c w) * P_i for every window w (W x the key size: ~6.4 GB for a 2^20 Groth16 key, which 80 GB of HBM affords).  All
 //    windows then share ONE bucket set, so there is no per-window reduction and no window-combine
 //    doubling chain on the per-proof path.
 //  * Per MSM: signed c-bit digits -> counting sort by bucket (histogram, scan, scatter) -> bucket
@@ -384,9 +384,8 @@ CS_GLOBAL void __launch_bounds__(128) k_msm_reduce_seg(const Xyzz<F>* __restrict
   red[t] = tot;
 }
 
-// A warp-shuffle version of this tree (five shuffle rounds per warp, then across the warps) was measured on B200 and
-// lost: every lane pays the full point addition in every round, and moving a 128/256-byte XYZZ point is 32/64 SHFL --
-// bucket reduction stage 0.399 ms against 0.329 ms for the tree below (profiles/r2_bench_final2_n1.json).
+// No warp-shuffle tree here: every lane would pay the full point addition in every round, and moving a 128/256-byte
+// XYZZ point is 32/64 SHFL, so a shuffle tree is slower than the shared-memory tree below.
 // Block b sums red[k] for k = b*T + t, stride gridDim.x*T, into out[b] (shared-memory tree); launched
 // twice: many blocks, then one block over the block results.
 template <class F>
@@ -506,14 +505,11 @@ static inline MsmShape msm_shape(uint32_t scalar_bits, uint32_t c) {
 }
 
 // Window size.  The work is W n mixed additions + ~4 * 2^(c-1) full additions in the bucket reduction
-// (running sums + the per-segment scalar multiple).  Measured on B200 at n = 2^20 (G1, dense):
-// c = 16: accumulate 2.90 ms, sort 0.42, fold+reduce 0.75;  c = 20: accumulate 2.34 ms but sort 1.32 and
-// fold+reduce 1.0 -- the 2^19-bucket phases eat the gain, so 16 stays the cap (window_bits overrides).
-// Below 2^15 points the window shrinks with the input (lg n - 4) so that tiny MSMs do not pay for 2^15 buckets;
-// from 2^15 on c = 16 wins (B200, G1: 2^16 points 0.75-0.84 ms at c = 15/16 vs 1.35 ms at c = 12; 2^18 points
-// 1.48 ms at c = 16 vs 2.92 ms at c = 14).  A window size whose TOP window is only a few bits wide is avoided:
-// its 2^k digit values send n / 2^k scalars each into the same handful of buckets and their fold becomes a
-// serial chain (the 2.9 ms case above: 254 + 1 = 18 * 14 + 3).
+// (running sums + the per-segment scalar multiple).  Wider windows cut the accumulation but the 2^(c-1)-bucket
+// phases (sort, fold, reduce) grow with them, so 16 is the cap (window_bits overrides).
+// Below 2^15 points the window shrinks with the input (lg n - 4) so that tiny MSMs do not pay for 2^15 buckets.
+// A window size whose TOP window is only a few bits wide is avoided: its 2^k digit values send n / 2^k scalars
+// each into the same handful of buckets and their fold becomes a serial chain (e.g. 254 + 1 = 18 * 14 + 3).
 static inline uint32_t msm_auto_window(size_t n, uint32_t scalar_bits) {
   int lg = 0;
   while ((1ull << (lg + 1)) <= n) lg++;
@@ -584,7 +580,7 @@ int msm_accum0_f52(const Affine<F>* table, const uint32_t* sorted, const uint32_
 // st_acc (optional): a second, LOWER-priority stream for the accumulation kernel alone.  When several MSMs share the
 // GPU, the block scheduler serves equal-priority grids in launch order, so the short sort / fold / reduce kernels of
 // one MSM queue behind the full-GPU accumulation grids of all the others (measured: folds of an MSM finished at 3 ms
-// ran at 13 ms, profiles/r2_prio_ab.log); with the accumulation on a lower-priority stream they slip in between.
+// ran long after their own accumulation); with the accumulation on a lower-priority stream they slip in between.
 template <class F, class FrP>
 int msm_enqueue(MsmWorkspace& ws, const Affine<F>* table, const uint32_t* infmask, uint32_t nbases, MsmShape sh,
                 uint32_t offset,
@@ -687,10 +683,10 @@ int msm_enqueue(MsmWorkspace& ws, const Affine<F>* table, const uint32_t* infmas
     st = st_acc;
   }
   {
-    // resident blocks per SM (register cap) -- tuned on B200, overridable for experiments
+    // resident blocks per SM (register cap), overridable for experiments
     static int minb_env = -1;
     if (minb_env < 0) { const char* e = getenv("CS_ACCUM0_MINB"); minb_env = e ? atoi(e) : 0; }
-    const int minb = minb_env ? minb_env : 4;  // B200, dense 2^20: G1 2.87 ms at 4 (2.95 at 5); G2 8.52 at 4, 8.72 at 3, 9.19 at 2, 8.78 at 5
+    const int minb = minb_env ? minb_env : 4;
     if (table_m260) {
       CS_TRY((msm_accum0_f52<F>(table, so.sorted.as<uint32_t>(), count, start, sstart0, nb1, S, order, order_b,
                                 ws.part0.as<Xyzz<F>>(), (uint32_t)max_s0, st)));

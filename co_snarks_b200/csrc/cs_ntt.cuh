@@ -206,7 +206,7 @@ int ntt_enqueue(uint32_t* d_data, const uint32_t* d_tw, uint32_t logn, uint32_t 
     uint32_t log_stride = dit ? done : (logn - done - k);
     bool last = (p + 1 == npass);
     uint32_t rows = 1u << k;
-    static int tws_env = -1, thr_env = -1;  // tuning hooks (profiles/r1_ntt_variant_sweep.jsonl)
+    static int tws_env = -1, thr_env = -1;  // tuning hooks
     if (tws_env < 0) { const char* e = getenv("CS_NTT_TWS"); tws_env = e ? atoi(e) : 1; }
     if (thr_env < 0) { const char* e = getenv("CS_NTT_THREADS"); thr_env = e ? atoi(e) : 512; }
     const bool tws = tws_env != 0;

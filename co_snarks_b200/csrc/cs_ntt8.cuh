@@ -12,7 +12,7 @@
 //  * butterflies run three stages at a time in registers (radix-8: 8 elements, 12 products, 7 twiddles per
 //    thread and round), so a 7-stage pass synchronises 3 times instead of 7 and touches shared memory 3 times.
 // Shared-memory bank conflicts are left alone on purpose: a butterfly costs ~600 issue cycles of Montgomery
-// product per warp (profiles/r2_pipe_probe.json), a 2-way conflicted LDS.128 pair ~16.
+// product per warp, a 2-way conflicted LDS.128 pair ~16.
 #pragma once
 #include "cs_common.cuh"
 #include "cs_field.cuh"

@@ -1,4 +1,4 @@
-// Carry-chain primitives for multi-limb integer arithmetic on sm_100a.
+// Carry-chain primitives for multi-limb integer arithmetic on sm_90a.
 //
 // Device build: one PTX instruction each (add.cc / addc.cc / mad.lo.cc / madc.hi.cc ...); ptxas fuses
 // mad.lo.cc + madc.hi.cc pairs into IMAD.WIDE.U32(.X) chains on the FMA pipe.

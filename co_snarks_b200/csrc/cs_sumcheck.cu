@@ -29,7 +29,7 @@ int fold_t(cs_ctx* ctx, const uint64_t* const* d_in, uint64_t* const* d_out, siz
   const uint32_t comps = shared ? 2 : 1;
   const size_t half = len / 2;
   unsigned blocks = ceil_div(half * comps, 256);
-  if (blocks > 148 * 8) blocks = 148 * 8;
+  if (blocks > CS_NUM_SMS * 8) blocks = CS_NUM_SMS * 8;
   for (size_t base = 0; base < n_polys; base += SC_FOLD_MAX) {
     const size_t cnt = n_polys - base < (size_t)SC_FOLD_MAX ? n_polys - base : (size_t)SC_FOLD_MAX;
     ScFoldArgs a;

@@ -1,4 +1,4 @@
-/* cosnarks_gpu.h -- C ABI of libcosnarks_gpu.so, the B200 (sm_100a) backend for the co-snarks hot path.
+/* cosnarks_gpu.h -- C ABI of libcosnarks_gpu.so, the H100 (sm_90a) backend for the co-snarks hot path.
  *
  * The reference (TaceoLabs/co-snarks @ 2b4592e) is pure Rust and has no FFI; its seams for this path
  * are (1) the crate `taceo-ark-algebra 0.1.0` (msm + fft), (2) the `R1CSToQAP` trait and (3) the
@@ -47,7 +47,7 @@ typedef struct cs_net cs_net; /* party-to-party transport, see "party-to-party t
 
 /* ---- library / context ------------------------------------------------------------------------ */
 const char* cs_last_error(void);
-/* version string, e.g. "cosnarks-b200 0.1 (sm_100a)" */
+/* version string, e.g. "cosnarks-b200 0.1 (sm_90a)" */
 const char* cs_version(void);
 /* `stream` = an existing cudaStream_t the context should run on (e.g. torch's current stream), or NULL
  * to let the context create its own. */

@@ -231,7 +231,7 @@ def reference_arm(log_m=20, target_log_m=20, steps=1, warmup=0):
             "dtype": "u64x4 (256-bit Montgomery, integer)",
             "data": "synthetic (same seeded R1CS as the GPU arm; timing-only key with the valid key's infinity pattern: "
                     "%.0f %% of the B-query bases are the point at infinity and are skipped by both arms)" % (100 * inf_frac),
-            "config": {"workload": "plain Groth16 prover, BN254, synthetic R1CS 2^%d constraints, 1xB200 per replica "
+            "config": {"workload": "plain Groth16 prover, BN254, synthetic R1CS 2^%d constraints, 1xH100 per replica "
                                    "(BASELINE.json configs[1])" % target_log_m, "arm": "host CPU (oracle/c port of the reference path)"},
             "cpu_baseline": {"value": v, "unit": "proofs/s", "cores": int(cores), "kind": "port", "sample": sample},
             "e2e": {"value": v, "unit": "proofs/s", "h2d_bytes_per_step": 0, "d2h_bytes_per_step": 0}}

@@ -1,8 +1,9 @@
 """Generates the golden fixtures under tests/golden/ from the reference's own test vectors.
 
-Run once in the build container (needs /root/reference, which does not exist on the GPU box):
-    python tests/golden/make_golden.py
-Inputs : /root/reference/test_vectors/{Groth16,Plonk}/... and co-noir-common/src/crs/bn254_g1.dat
+Run once where the reference tree is available (REF below):
+    python tests/golden/make_golden.py       # the JSON fixtures
+    python tests/golden/make_golden.py raw   # the reference's own fixture files, gzipped under golden/reference/
+Inputs : the reference tree's test_vectors/{Groth16,Plonk}/... and co-noir/co-noir-common/src/crs/bn254_g1.dat
 Expected values:
   * Plonk round-1 commitments are the REFERENCE'S known answers, typed in from
     co-circom/co-plonk/src/round1.rs:351-371 (BN254 multiplier2) and :397-417 (BLS12-381 poseidon);
@@ -224,7 +225,39 @@ def crs_fixture(n):
                                           points=[p1(P) for P in pts]), True)
 
 
+# The reference's fixture files that tests read as files (parsers, .zkey / .wtns ingest), gzipped byte for byte.
+# CRS: the first 64 points of bn254_g1.dat only.
+RAW_FILES = [
+    ("test_vectors/Groth16/bn254/multiplier2/" + f, None) for f in ("circuit.zkey", "witness.wtns")
+] + [
+    ("test_vectors/Groth16/bn254/poseidon/" + f, None) for f in ("circuit.zkey", "witness.wtns", "verification_key.json")
+] + [
+    ("test_vectors/Groth16/bls12_381/poseidon/" + f, None)
+    for f in ("circuit.zkey", "witness.wtns", "verification_key.json", "public.json", "circom.proof")
+] + [
+    ("test_vectors/Plonk/bls12_381/poseidon/" + f, None) for f in ("verification_key.json", "public.json", "circom.proof")
+] + [
+    ("test_vectors/Plonk/%s/multiplier2/circuit.zkey" % c, None) for c in ("bn254", "bls12_381")
+] + [
+    ("co-noir/co-noir-common/src/crs/bn254_g1.dat", 64 * 64),
+]
+
+
+def raw_files():
+    for rel, nbytes in RAW_FILES:
+        with open(os.path.join(REF, rel), "rb") as f:
+            data = f.read() if nbytes is None else f.read(nbytes)
+        path = os.path.join(HERE, "reference", rel + ".gz")
+        os.makedirs(os.path.dirname(path), exist_ok=True)
+        with gzip.GzipFile(path, "wb", mtime=0) as f:
+            f.write(data)
+        print(path, os.path.getsize(path))
+
+
 if __name__ == "__main__":
+    if sys.argv[1:] == ["raw"]:
+        raw_files()
+        sys.exit(0)
     groth16_fixture("multiplier2", [(0, 0), (5, 7)], False)
     groth16_fixture("poseidon", [(123456789, 987654321)], True)
     plonk_fixture("bn254", "multiplier2", [

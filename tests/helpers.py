@@ -19,6 +19,15 @@ def load_golden(name):
         return json.loads(f.read().decode())
 
 
+def reference_file(rel, out_dir):
+    """One of the reference's own fixture files (stored gzipped under golden/reference/ by make_golden.py raw),
+    unpacked into out_dir; rel is its path in the reference tree.  Returns the unpacked file's path."""
+    path = os.path.join(str(out_dir), rel.replace("/", "__"))
+    with gzip.open(os.path.join(GOLDEN, "reference", rel + ".gz"), "rb") as f, open(path, "wb") as o:
+        o.write(f.read())
+    return path
+
+
 def ih(x):
     return int(x, 16)
 

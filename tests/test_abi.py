@@ -29,7 +29,7 @@ def test_header_declares_and_library_exports_every_symbol():
 
 def test_version_string():
     lib = B.load()
-    assert b"sm_100a" in lib.cs_version()
+    assert b"sm_90a" in lib.cs_version()
 
 
 def test_no_cpu_fallback_without_gpu():

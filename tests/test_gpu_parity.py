@@ -1,4 +1,4 @@
-"""GPU parity tests (run with -m gpu on a B200 via gpurun): libcosnarks_gpu.so through the C ABI against
+"""GPU parity tests (run with -m gpu on an H100): libcosnarks_gpu.so through the C ABI against
 the oracle / golden vectors.  Bit-exact: all arithmetic is integer."""
 import pytest
 

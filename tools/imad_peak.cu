@@ -1,7 +1,7 @@
 // Integer-pipe microbenchmark for the MSM/NTT roofline: sustained IMAD (32x32+32) and IMAD.WIDE
-// (32x32+64) issue rate on B200, and the throughput of the library's Montgomery multiplication.
-// MEASURED_PEAKS.json only carries HBM and bf16 peaks; 256-bit modular arithmetic is bound by this
-// pipe instead (DESIGN.md "Rooflines").  Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3
+// (32x32+64) issue rate on H100, and the throughput of the library's Montgomery multiplication.
+// HBM and tensor-core peaks say nothing here: 256-bit modular arithmetic is bound by this
+// pipe instead (DESIGN.md "Rooflines").  Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3
 #include <cstdio>
 #include <cstdint>
 #include <cuda_runtime.h>

@@ -1,4 +1,4 @@
-"""Extracts the judged subset of an .ncu-rep (ncu -i ... --page raw --csv) into a small CSV under profiles/."""
+"""Extracts the judged subset of an .ncu-rep (ncu -i ... --page raw --csv) into a small CSV."""
 import csv
 import subprocess
 import sys

@@ -1,4 +1,4 @@
-// Issue-rate probe for the pipes a 256-bit modular multiplication can use on B200 (sm_100a):
+// Issue-rate probe for the pipes a 256-bit modular multiplication can use on H100 (sm_90a):
 //   * IMAD.WIDE.U32 without carries, with carry-out only, and the carry-in/out (.X) form the CIOS product uses
 //   * DFMA (FP64 pipe) alone and interleaved with IMAD.WIDE -- do the two pipes overlap?
 //   * IADD3 / IADD3.X (ALU pipe) alone and interleaved with IMAD.WIDE

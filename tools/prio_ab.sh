@@ -1,7 +1,7 @@
 #!/bin/bash
 # A/B of the prover's stream layout with the stage timeline of one proof.  CS_PRIO="side,acc,wm" = CUDA priorities of the
 # MSM streams (sort / fold / reduce), of the accumulation streams and of the witness-map -> H stream; CS_MSM_SPLIT=0 keeps
-# each MSM on one stream.  usage (on the GPU box): bash tools/prio_ab.sh > gpurun_out/r2_prio_ab2.log
+# each MSM on one stream.  usage: bash tools/prio_ab.sh > prio_ab.log
 run() {
   echo "== $*"
   env "$@" timeout 300 python bench.py --steps 10 --warmup 3 --no-rep3 --no-cpu-baseline --timeline 2>&1 \

@@ -1,7 +1,7 @@
 """SASS opcode summary of the shipped kernels (cuobjdump -sass of co_snarks_b200/libcosnarks_gpu.so), per kernel:
 instruction count, the dominant opcodes, local-memory traffic (LDL / STL = spills or stack arrays) and the
 Blackwell / Hopper-era mnemonics the profiling recipe names (UBLKCP = cp.async.bulk, SYNCS = mbarrier, UTMALDG /
-UTMASTG = tensor-map TMA, DFMA, IMAD.WIDE).  usage: sass_summary.py [lib.so] > profiles/rN_sass_summary.md"""
+UTMASTG = tensor-map TMA, DFMA, IMAD.WIDE).  usage: sass_summary.py [lib.so] > sass_summary.md"""
 import collections
 import re
 import subprocess
@@ -24,7 +24,7 @@ for line in out.splitlines():
         kern[cur][m.group(1)] += 1
 demangle = subprocess.run(["c++filt"], input="\n".join(kern), capture_output=True, text=True).stdout.splitlines()
 WATCH = ("UBLKCP", "SYNCS", "UTMALDG", "UTMASTG", "DFMA", "SHFL", "LDL", "STL", "ATOMG", "RED", "LDGSTS")
-print("# SASS summary of %s (sm_100a)\n" % LIB)
+print("# SASS summary of %s (sm_90a)\n" % LIB)
 print("Opcode classes counted per kernel body incl. its out-of-line device functions; `local` = LDL + STL.\n")
 print("| kernel | instr | IMAD.WIDE* | IMAD* other | DFMA+DADD | ALU (IADD3/LOP3/SHF/SEL/..) | local | TMA/mbarrier | top opcodes |")
 print("|---|---|---|---|---|---|---|---|---|")

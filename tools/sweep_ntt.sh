@@ -1,13 +1,11 @@
 #!/bin/bash
-# sweeps the NTT tuning hooks; one JSON line per variant into gpurun_out/ntt_sweep.jsonl
-mkdir -p gpurun_out
-: > gpurun_out/ntt_sweep.jsonl
+# sweeps the NTT tuning hooks; one JSON line per variant on stdout.  usage: bash tools/sweep_ntt.sh > ntt_sweep.jsonl
 for tws in 0 1; do
   for thr in 512 256 128; do
     for minb in 1; do
       if [ $minb = 3 ] && [ $thr != 512 ]; then continue; fi
-      echo "tws=$tws thr=$thr minb=$minb" >> gpurun_out/ntt_sweep.jsonl
-      CS_NTT_TWS=$tws CS_NTT_THREADS=$thr CS_NTT_MINB=$minb timeout 300 python tools/time_ntt.py >> gpurun_out/ntt_sweep.jsonl 2>&1
+      echo "tws=$tws thr=$thr minb=$minb"
+      CS_NTT_TWS=$tws CS_NTT_THREADS=$thr CS_NTT_MINB=$minb timeout 300 python tools/time_ntt.py 2>&1
     done
   done
 done

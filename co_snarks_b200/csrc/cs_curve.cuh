@@ -24,16 +24,58 @@ struct Fp2 {
   CS_D bool operator!=(const Fp2& b) const { return !(*this == b); }
   friend CS_D Fp2 operator+(const Fp2& a, const Fp2& b) { Fp2 r; r.c0 = a.c0 + b.c0; r.c1 = a.c1 + b.c1; return r; }
   friend CS_D Fp2 operator-(const Fp2& a, const Fp2& b) { Fp2 r; r.c0 = a.c0 - b.c0; r.c1 = a.c1 - b.c1; return r; }
-  // mul / sqr are out-of-line (one copy per kernel) to keep the G2 point formulas in the I-cache.
+  // mul / sqr / mul_sub are out-of-line (one copy per kernel) to keep the G2 point formulas in the I-cache.
   friend CS_D Fp2 operator*(const Fp2& a, const Fp2& b) { return mul_ool(a, b); }
+  // Karatsuba on unreduced 2N-word products with one Montgomery reduction per coefficient: 5 N^2 wide multiply-adds
+  // instead of the 6 N^2 of three reduced products.
+  //   v0 = a0 b0, v1 = a1 b1 < p^2;  v2 = (a0 + a1)(b0 + b1) < 4 p^2 (sums < 2p, left unreduced)
+  //   c1 = v2 - v0 - v1 = a0 b1 + a1 b0 < 2 p^2;  c0 = v0 + p^2 - v1 in (0, 2 p^2)
+  // F::redc needs its input below p 2^(32N): 2 p^2 is, since 2 p < 2^(32N).
   static CS_DN Fp2 mul_ool(Fp2 a, Fp2 b) {
-    // Karatsuba: 3 base multiplications, inlined HERE (not three calls) so that ptxas can interleave the
-    // three independent carry chains: the G2 kernels run at 2-3 resident blocks and need the ILP
-    F v0 = F::mul_inline(a.c0, b.c0), v1 = F::mul_inline(a.c1, b.c1);
-    F v2 = F::mul_inline(a.c0 + a.c1, b.c0 + b.c1);
+    constexpr int W = 2 * P::N;
+    uint32_t v0[W], v1[W], v2[W];
+    F::mul_wide(v0, a.c0, b.c0);
+    F::mul_wide(v1, a.c1, b.c1);
+    F::mul_wide(v2, F::add_unreduced(a.c0, a.c1), F::add_unreduced(b.c0, b.c1));
+    sub_n<W>(v2, v0);
+    sub_n<W>(v2, v1);
+    add_mod_sq<P, 1>(v0);
+    sub_n<W>(v0, v1);
     Fp2 r;
-    r.c1 = v2 - v0 - v1;
-    r.c0 = v0 - v1;
+    r.c0 = F::redc(v0);
+    r.c1 = F::redc(v2);
+    return r;
+  }
+  // a b - c d with two Montgomery reductions (8 N^2 wide multiply-adds instead of the 12 N^2 of two reduced Fp2
+  // products and a subtraction).  With u = the Karatsuba products of a b and w those of c d (as in mul_ool):
+  //   t0 = 2 p^2 + (u0 - u1) - (w0 - w1)                       in (0, 4 p^2): both differences lie in (-p^2, p^2)
+  //   t1 = 2 p^2 + (u2 - u0 - u1) - (w2 - w0 - w1)            in (0, 4 p^2): both cross sums lie in [0, 2 p^2)
+  // The partial sums may wrap modulo 2^(64N); the totals do not.  F::redc needs t < p 2^(32N), i.e. 4 p < 2^(32N):
+  // 2^256 / q = 5.3 for BN254 and 2^384 / p = 9.8 for BLS12-381.
+  static CS_DN Fp2 mul_sub_ool(Fp2 a, Fp2 b, Fp2 c, Fp2 d) {
+    constexpr int W = 2 * P::N;
+    uint32_t t0[W], t1[W], t[W];
+    CS_UNROLL
+    for (int i = 0; i < W; i++) t0[i] = t1[i] = mod_sq<P, 2>(i);
+    F::mul_wide(t, a.c0, b.c0);  // u0
+    add_n<W>(t0, t);
+    sub_n<W>(t1, t);
+    F::mul_wide(t, a.c1, b.c1);  // u1
+    sub_n<W>(t0, t);
+    sub_n<W>(t1, t);
+    F::mul_wide(t, F::add_unreduced(a.c0, a.c1), F::add_unreduced(b.c0, b.c1));  // u2
+    add_n<W>(t1, t);
+    F::mul_wide(t, c.c0, d.c0);  // w0
+    sub_n<W>(t0, t);
+    add_n<W>(t1, t);
+    F::mul_wide(t, c.c1, d.c1);  // w1
+    add_n<W>(t0, t);
+    add_n<W>(t1, t);
+    F::mul_wide(t, F::add_unreduced(c.c0, c.c1), F::add_unreduced(d.c0, d.c1));  // w2
+    sub_n<W>(t1, t);
+    Fp2 r;
+    r.c0 = F::redc(t0);
+    r.c1 = F::redc(t1);
     return r;
   }
   CS_D Fp2 sqr() const { return sqr_ool(*this); }
@@ -56,11 +98,13 @@ struct Fp2 {
   }
 };
 
-// a b - c d: one fused reduction in the base field (Fp::dot2), two products in the extension
+// a b - c d: one fused reduction in the base field (Fp::dot2), one per coefficient in the extension
 template <class P>
 CS_D Fp<P> mul_sub(const Fp<P>& a, const Fp<P>& b, const Fp<P>& c, const Fp<P>& d) { return Fp<P>::dot2(a, b, c.neg(), d); }
 template <class P>
-CS_D Fp2<P> mul_sub(const Fp2<P>& a, const Fp2<P>& b, const Fp2<P>& c, const Fp2<P>& d) { return a * b - c * d; }
+CS_D Fp2<P> mul_sub(const Fp2<P>& a, const Fp2<P>& b, const Fp2<P>& c, const Fp2<P>& d) {
+  return Fp2<P>::mul_sub_ool(a, b, c, d);
+}
 
 // Affine point; (0, 0) encodes infinity (never on y^2 = x^3 + b with b != 0) -- the same marker
 // snarkjs .zkey files use.

@@ -76,6 +76,78 @@ CS_D void mad_n_redc(uint32_t* X, uint32_t* Y, const uint32_t* a, uint32_t bi) {
   Y[N - 1] = addc(Y[N - 1], 0);
 }
 
+// The product half of a mad_n_redc row (the unreduced product Fp::mul_wide): X gets the low word of the shifted value
+template <int N>
+CS_D void mad_n(uint32_t* X, uint32_t* Y, const uint32_t* a, uint32_t bi) {
+  X[0] = add_cc(X[0], Y[1]);
+  madc_n_rshift<N>(Y, a + 1, bi);
+  cmad_n<N>(X, a, bi);
+  Y[N - 1] = addc(Y[N - 1], 0);
+}
+// A row of the reduction alone (Fp::redc): the one-word shift of mad_n_redc moves into the chain that adds m p
+template <class P>
+CS_D void redc_row(uint32_t* X, uint32_t* Y, const uint32_t* mod) {
+  constexpr int N = P::N;
+  const uint32_t m = mul_lo(X[0] + Y[1], P::M0);
+  X[0] = add_cc(X[0], Y[1]);
+  madc_n_rshift<N>(Y, mod + 1, m);
+  cmad_n<N>(X, mod, m);
+  Y[N - 1] = addc(Y[N - 1], 0);
+}
+
+// r[0..M) += a[0..M)  /  r[0..M) -= a[0..M), modulo 2^(32 M)
+template <int M>
+CS_D void add_n(uint32_t* r, const uint32_t* a) {
+  r[0] = add_cc(r[0], a[0]);
+  CS_UNROLL
+  for (int i = 1; i < M - 1; i++) r[i] = addc_cc(r[i], a[i]);
+  r[M - 1] = addc(r[M - 1], a[M - 1]);
+}
+template <int M>
+CS_D void sub_n(uint32_t* r, const uint32_t* a) {
+  r[0] = sub_cc(r[0], a[0]);
+  CS_UNROLL
+  for (int i = 1; i < M - 1; i++) r[i] = subc_cc(r[i], a[i]);
+  r[M - 1] = subc(r[M - 1], a[M - 1]);
+}
+
+// K p^2 as 2N little-endian words, evaluated by the compiler: the offsets that keep the lazy Fp2 sums non-negative
+template <class P, int K>
+struct ModSq {
+  uint32_t v[2 * P::N];
+  CS_HD constexpr ModSq() : v{} {
+    for (int i = 0; i < P::N; i++) {
+      uint64_t carry = 0;
+      for (int j = 0; j < P::N; j++) {
+        const uint64_t s = (uint64_t)P::mod(i) * P::mod(j) + v[i + j] + carry;
+        v[i + j] = (uint32_t)s;
+        carry = s >> 32;
+      }
+      v[i + P::N] = (uint32_t)carry;
+    }
+    uint64_t carry = 0;
+    for (int k = 0; k < 2 * P::N; k++) {
+      const uint64_t s = (uint64_t)v[k] * K + carry;
+      v[k] = (uint32_t)s;
+      carry = s >> 32;
+    }
+  }
+};
+template <class P, int K>
+CS_HD constexpr uint32_t mod_sq(int k) {
+  constexpr ModSq<P, K> t;
+  return t.v[k];
+}
+// r[0..2N) += K p^2
+template <class P, int K>
+CS_D void add_mod_sq(uint32_t* r) {
+  constexpr int M = 2 * P::N;
+  r[0] = add_cc(r[0], mod_sq<P, K>(0));
+  CS_UNROLL
+  for (int i = 1; i < M - 1; i++) r[i] = addc_cc(r[i], mod_sq<P, K>(i));
+  r[M - 1] = addc(r[M - 1], mod_sq<P, K>(M - 1));
+}
+
 template <class P>
 struct Fp {
   static constexpr int N = P::N;
@@ -258,6 +330,68 @@ struct Fp {
       c0 = c1; c1 = c2; c2 = 0;
     }
     r.l[N - 1] = c0;
+    r.final_sub();
+    return r;
+  }
+
+  // ---- lazy reduction (the Fp2 products of cs_curve.cuh): an unreduced product and a separate reduction
+  // a + b without the final subtraction: < 2p, which still fits N words (2p < 2^(32N) for every modulus here)
+  static CS_D Fp add_unreduced(const Fp& a, const Fp& b) {
+    Fp r;
+    r.l[0] = add_cc(a.l[0], b.l[0]);
+    CS_UNROLL
+    for (int i = 1; i < N - 1; i++) r.l[i] = addc_cc(a.l[i], b.l[i]);
+    r.l[N - 1] = addc(a.l[N - 1], b.l[N - 1]);
+    return r;
+  }
+  // t[0..2N) = a b, unreduced, for a < 2^(32N - 1) (an unreduced sum < 2p qualifies) and any N-word b.  The rows of
+  // mul_inline without their reduction halves: N^2 wide multiply-adds in one carry chain per half-row, and the word
+  // that leaves the bottom of each row is the next word of t.
+  static CS_D void mul_wide(uint32_t* t, const Fp& a, const Fp& b) {
+    uint32_t even[N], odd[N];
+    mul_n<N>(odd, a.l + 1, b.l[0]);
+    mul_n<N>(even, a.l, b.l[0]);
+    t[0] = even[0];
+    CS_UNROLL
+    for (int i = 1; i < N; i += 2) {
+      mad_n<N>(odd, even, a.l, b.l[i]);
+      t[i] = odd[0];
+      if (i + 1 < N) {
+        mad_n<N>(even, odd, a.l, b.l[i + 1]);
+        t[i + 1] = even[0];
+      }
+    }
+    // t[N..2N) = even + (odd >> 32)
+    t[N] = add_cc(even[0], odd[1]);
+    CS_UNROLL
+    for (int k = 1; k < N - 1; k++) t[N + k] = addc_cc(even[k], odd[k + 1]);
+    t[2 * N - 1] = addc(even[N - 1], 0);
+  }
+  // t R^-1 mod p (R = 2^(32N)) of a 2N-word t < p R, fully reduced.  The reduction rows of mul_inline run over the
+  // low half (N^2 wide multiply-adds; the shift of each row rides in its reduction chain), which leaves
+  // (t_lo + m p) / R <= p; adding t_hi < p stays below 2p, so one final subtraction suffices.
+  static CS_D Fp redc(const uint32_t* t) {
+    uint32_t even[N], odd[N], mod[N];
+    CS_UNROLL
+    for (int i = 0; i < N; i++) { even[i] = t[i]; mod[i] = P::mod(i); }
+    const uint32_t m = mul_lo(even[0], P::M0);
+    mul_n<N>(odd, mod + 1, m);
+    cmad_n<N>(even, mod, m);
+    odd[N - 1] = addc(odd[N - 1], 0);
+    CS_UNROLL
+    for (int i = 1; i < N; i += 2) {
+      redc_row<P>(odd, even, mod);
+      if (i + 1 < N) redc_row<P>(even, odd, mod);
+    }
+    Fp r;
+    r.l[0] = add_cc(even[0], odd[1]);
+    CS_UNROLL
+    for (int k = 1; k < N - 1; k++) r.l[k] = addc_cc(even[k], odd[k + 1]);
+    r.l[N - 1] = addc(even[N - 1], 0);
+    r.l[0] = add_cc(r.l[0], t[N]);
+    CS_UNROLL
+    for (int k = 1; k < N - 1; k++) r.l[k] = addc_cc(r.l[k], t[N + k]);
+    r.l[N - 1] = addc(r.l[N - 1], t[2 * N - 1]);
     r.final_sub();
     return r;
   }

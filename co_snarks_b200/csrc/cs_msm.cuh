@@ -308,6 +308,20 @@ CS_GLOBAL void __launch_bounds__(128, MINB) k_msm_accum0(const Affine<F>* __rest
   if (end > beg + S) end = beg + S;
   Xyzz<F> acc = Xyzz<F>::inf();
   uint32_t e = sorted[beg];
+  if constexpr (sizeof(Affine<F>) > 64) {
+    // G2: the 64-register accumulator leaves no room for a register copy of the next 128-byte point, so the next point
+    // is only prefetched into L1 (no registers held) and loaded when its addition starts
+    for (uint32_t k = beg; k < end; k++) {
+      const uint32_t e_cur = e;
+      if (k + 1 < end) {
+        e = sorted[k + 1];
+        prefetch_l1(table + (e & ~MSM_SIGN));
+      }
+      madd(acc, table[e_cur & ~MSM_SIGN], (e_cur & MSM_SIGN) != 0);
+    }
+    part0[s] = acc;
+    return;
+  }
   Affine<F> p = table[e & ~MSM_SIGN];
   for (uint32_t k = beg; k < end; k++) {
     uint32_t e_cur = e;
@@ -683,10 +697,11 @@ int msm_enqueue(MsmWorkspace& ws, const Affine<F>* table, const uint32_t* infmas
     st = st_acc;
   }
   {
-    // resident blocks per SM (register cap), overridable for experiments
+    // resident blocks per SM (register cap), overridable for experiments.  G2 at 2: the cap under which its kernel does
+    // not spill, and the fastest in a sweep on the H100 (DESIGN.md 4.2)
     static int minb_env = -1;
     if (minb_env < 0) { const char* e = getenv("CS_ACCUM0_MINB"); minb_env = e ? atoi(e) : 0; }
-    const int minb = minb_env ? minb_env : 4;
+    const int minb = minb_env ? minb_env : (sizeof(Affine<F>) > 64 ? 2 : 4);
     if (table_m260) {
       CS_TRY((msm_accum0_f52<F>(table, so.sorted.as<uint32_t>(), count, start, sstart0, nb1, S, order, order_b,
                                 ws.part0.as<Xyzz<F>>(), (uint32_t)max_s0, st)));

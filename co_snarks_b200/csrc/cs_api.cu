@@ -121,6 +121,7 @@ void cs_ctx_destroy(cs_ctx* ctx) {
   if (!ctx) return;
   cudaSetDevice(ctx->device);
   cudaDeviceSynchronize();
+  ctx->msm_ws[CS_WIT_SORT].release();
   for (int i = 0; i < CS_NSIDE; i++) {
     ctx->msm_ws[i].release();
     if (ctx->side[i]) cudaStreamDestroy(ctx->side[i]);
@@ -221,11 +222,11 @@ int bases_upload_t(cs_ctx* ctx, const uint64_t* h_points, size_t n, int window_b
 
 template <class Cfg, int G>
 int msm_enqueue_t(cs_ctx* ctx, int slot, cudaStream_t st, const cs_bases* b, size_t offset,
-                  const uint32_t* d_scalars, unsigned sstride, size_t n, int mont, int sort_slot) {
+                  const uint32_t* d_scalars, unsigned sstride, size_t n, int mont, int sort_slot, bool view) {
   typedef typename GroupOf<Cfg, G>::F F;
   return msm_enqueue<F, typename Cfg::FrP>(ctx->msm_ws[slot], b->table.as<Affine<F>>(), b->infmask.as<uint32_t>(), (uint32_t)b->n, b->sh,
                                            (uint32_t)offset, d_scalars, sstride, (uint32_t)n, mont, st,
-                                           sort_slot >= 0 ? &ctx->msm_ws[sort_slot] : nullptr, b->m260, ctx->acc[slot]);
+                                           sort_slot >= 0 ? &ctx->msm_ws[sort_slot] : nullptr, view, b->m260, ctx->acc[slot]);
 }
 
 // After the stream has drained: XYZZ (pinned) -> affine on the host.
@@ -239,22 +240,19 @@ void msm_finish_t(cs_ctx* ctx, int slot, uint64_t* out_affine, int* out_inf) {
 }
 
 int msm_enqueue_dyn(cs_ctx* ctx, int slot, cudaStream_t st, const cs_bases* b, size_t offset,
-                    const uint32_t* d_scalars, unsigned sstride, size_t n, int mont, int sort_slot) {
+                    const uint32_t* d_scalars, unsigned sstride, size_t n, int mont, int sort_slot, bool view) {
   CS_DISPATCH_CURVE(b->curve, {
-    if (b->group == CS_G1) return msm_enqueue_t<Cfg, 0>(ctx, slot, st, b, offset, d_scalars, sstride, n, mont, sort_slot);
-    return msm_enqueue_t<Cfg, 1>(ctx, slot, st, b, offset, d_scalars, sstride, n, mont, sort_slot);
+    if (b->group == CS_G1) return msm_enqueue_t<Cfg, 0>(ctx, slot, st, b, offset, d_scalars, sstride, n, mont, sort_slot, view);
+    return msm_enqueue_t<Cfg, 1>(ctx, slot, st, b, offset, d_scalars, sstride, n, mont, sort_slot, view);
   });
   return 0;
 }
-int bases_sort_compatible(cs_ctx* ctx, const cs_bases* a, const cs_bases* b, bool* out) {
-  *out = false;
-  if (!a || !b || a->curve != b->curve || a->n != b->n || a->sh.c != b->sh.c || a->sh.W != b->sh.W) return 0;
-  const size_t words = (a->n + 31) / 32;
-  std::vector<uint32_t> ma(words), mb(words);
-  CS_CUDA(cudaMemcpyAsync(ma.data(), a->infmask.p, words * 4, cudaMemcpyDeviceToHost, ctx->stream));
-  CS_CUDA(cudaMemcpyAsync(mb.data(), b->infmask.p, words * 4, cudaMemcpyDeviceToHost, ctx->stream));
-  CS_CUDA(cudaStreamSynchronize(ctx->stream));
-  *out = ma == mb;
+int msm_sort_shared_dyn(cs_ctx* ctx, int slot, cudaStream_t st, const cs_bases* b, const uint32_t* d_scalars,
+                        unsigned sstride, size_t n, int mont) {
+  CS_DISPATCH_CURVE(b->curve, {
+    return msm_sort<typename Cfg::FrP>(ctx->msm_ws[slot], nullptr, (uint32_t)n, b->sh, 0, d_scalars, sstride, (uint32_t)n,
+                                       mont, st);
+  });
   return 0;
 }
 

@@ -27,7 +27,10 @@ struct cs_groth16_pk {
   // LibSnarkReduction (reduction.rs:241-342): C matrix, arkworks domain, coset = GENERATOR
   DevBuf c_rowptr, c_col, c_coeff;
   bool have_c = false;
-  bool share_b_sort = false;  // B1 and B2 sort identically (same infinity pattern): B2 reuses B1's sorted entries
+  // Whose sorted entries each witness MSM (A, B1, B2, L) accumulates, decided once from the infinity masks
+  // (plan_witness_views): -1 = the shared witness sort as it is; its own index = its own filtered view of that sort;
+  // another index = that MSM's view (same table geometry and infinity pattern, as B2 has with B1)
+  int wit_src[4] = {0, 1, 2, 3};
   cs_domain* dom_ark = nullptr;
   DevBuf coset_tab_ark, ginv_pows, vinv_over_n;
 };
@@ -241,6 +244,43 @@ int witness_map_libsnark_device(cs_ctx* ctx, cs_groth16_pk* pk, int kind, int pa
   return 0;
 }
 
+// Fills pk->wit_src.  A witness MSM reads the shared witness sort as it is when its table slots are that sort's
+// entries (w * nw + i: nw bases, offset 0) and none of its bases is infinite -- L of a key in which every witness
+// variable occurs.  Any other MSM filters the sort for its table, and MSMs whose tables agree in length, offset and
+// infinity pattern share one filtered view (B1 and B2: B_i(tau) G1 and B_i(tau) G2 vanish together).
+int plan_witness_views(cs_ctx* ctx, cs_groth16_pk* pk) {
+  const size_t ni = pk->ni, nw = pk->nw;
+  if (!nw) return 0;
+  const cs_bases* q[4] = {pk->a_query, pk->b_g1, pk->b_g2, pk->l_query};
+  const size_t off[4] = {ni, ni, ni, 0};
+  std::vector<uint8_t> inf[4];
+  for (int j = 0; j < 4; j++) {
+    if (q[j]->sh.c != q[0]->sh.c || q[j]->sh.W != q[0]->sh.W)
+      return fail(CS_ERR_STATE, "cs_groth16_pk_create: the witness MSMs' tables differ in window shape");
+    std::vector<uint32_t> words((q[j]->n + 31) / 32);
+    CS_CUDA(cudaMemcpyAsync(words.data(), q[j]->infmask.p, words.size() * 4, cudaMemcpyDeviceToHost, ctx->stream));
+    CS_CUDA(cudaStreamSynchronize(ctx->stream));
+    inf[j].resize(nw);
+    bool any = false;
+    for (size_t i = 0; i < nw; i++) {
+      const size_t k = off[j] + i;
+      inf[j][i] = (words[k >> 5] >> (k & 31)) & 1;
+      any = any || inf[j][i];
+    }
+    pk->wit_src[j] = j;
+    if (q[j]->n == nw && off[j] == 0 && !any) {
+      pk->wit_src[j] = -1;
+      continue;
+    }
+    for (int k = 0; k < j; k++)
+      if (pk->wit_src[k] == k && q[k]->n == q[j]->n && off[k] == off[j] && inf[k] == inf[j]) {
+        pk->wit_src[j] = k;
+        break;
+      }
+  }
+  return 0;
+}
+
 int upload_inputs(cs_ctx* ctx, cs_groth16_pk* pk, int kind, const uint64_t* h_pub, const uint64_t* h_wit,
                   const uint64_t* h_m1, const uint64_t* h_m2) {
   const unsigned batch = kind == CS_REP3 ? 2 : 1;
@@ -274,7 +314,7 @@ int local_phase(cs_ctx* ctx, cs_groth16_pk* pk, int kind, int party, const uint6
   // (6-10 NTTs, then a full MSM), so it is enqueued FIRST and on the highest-priority stream: its passes interleave
   // with the other MSMs' accumulation grids instead of queueing behind all of them (otherwise H starts only after the
   // four side MSMs have drained).
-  CS_TRY(ctx_fork(ctx, 4));
+  CS_TRY(ctx_fork(ctx, 5));
   cudaStream_t wm = ctx->wm;
   CS_CUDA(cudaStreamWaitEvent(wm, ctx->ev_fork, 0));
   // witness either uploaded from the host just above, or already resident in HBM (d_wit_in)
@@ -306,14 +346,22 @@ int local_phase(cs_ctx* ctx, cs_groth16_pk* pk, int kind, int party, const uint6
   if (have_aux) {
     // query[1 + pub_len ..] = query[ni ..]  (groth16.rs:193)
     CS_SPAN("compute A, B/G1, B/G2 in create proof with assignment + msm l_query");
-    if (do_a) CS_TRY(msm_enqueue_dyn(ctx, 0, ctx->side[0], pk->a_query, pk->ni, wit, batch, pk->nw, 1));
-    if (do_b1) CS_TRY(msm_enqueue_dyn(ctx, 1, ctx->side[1], pk->b_g1, pk->ni, wit, batch, pk->nw, 1));
-    if (do_b2)
-      CS_TRY(msm_enqueue_dyn(ctx, 2, ctx->side[2], pk->b_g2, pk->ni, wit, batch, pk->nw, 1,
-                             (do_b1 && pk->share_b_sort) ? 1 : -1));
-    if (do_l) CS_TRY(msm_enqueue_dyn(ctx, 3, ctx->side[3], pk->l_query, 0, wit, batch, pk->nw, 1));
+    // the four MSMs take the same scalars: their digits are sorted once, on side stream 4, and each MSM reads that
+    // sort as it is or filters it for its own table (msm_enqueue)
+    const unsigned part[4] = {CS_PART_A, CS_PART_B1, CS_PART_B2, CS_PART_L};
+    const cs_bases* q[4] = {pk->a_query, pk->b_g1, pk->b_g2, pk->l_query};
+    const size_t off[4] = {pk->ni, pk->ni, pk->ni, 0};
+    if (do_a || do_b1 || do_b2 || do_l)
+      CS_TRY(msm_sort_shared_dyn(ctx, CS_WIT_SORT, ctx->side[4], pk->a_query, wit, batch, pk->nw, 1));
+    for (int j = 0; j < 4; j++) {
+      if (!(parts & part[j])) continue;
+      int src = pk->wit_src[j];
+      if (src >= 0 && !(parts & part[src])) src = j;  // the MSM that builds the view is not part of this call
+      const int sort_slot = src < 0 || src == j ? CS_WIT_SORT : src;
+      CS_TRY(msm_enqueue_dyn(ctx, j, ctx->side[j], q[j], off[j], wit, batch, pk->nw, 1, sort_slot, src == j));
+    }
   }
-  CS_TRY(ctx_join(ctx, 4));
+  CS_TRY(ctx_join(ctx, 5));
   CS_CUDA(cudaEventRecord(ctx->ev_wm, wm));
   CS_CUDA(cudaStreamWaitEvent(ctx->stream, ctx->ev_wm, 0));
 
@@ -678,16 +726,16 @@ int cs_groth16_pk_create(cs_ctx* ctx, const cs_groth16_key_desc* d, cs_groth16_p
   pk->b2_head.assign(d->b_g2_query, d->b_g2_query + ni * 4 * fq);
   (void)g1b; (void)g2b;
   const int wb = d->window_bits;
-  CS_TRY(cs_bases_upload(ctx, d->curve, CS_G1, d->a_query, d->a_query_len, wb, &pk->a_query));
-  CS_TRY(cs_bases_upload(ctx, d->curve, CS_G1, d->b_g1_query, d->b_g1_query_len, wb, &pk->b_g1));
-  CS_TRY(cs_bases_upload(ctx, d->curve, CS_G2, d->b_g2_query, d->b_g2_query_len, wb, &pk->b_g2));
-  if (nw) CS_TRY(cs_bases_upload(ctx, d->curve, CS_G1, d->l_query, d->l_query_len, wb, &pk->l_query));
+  // A, B1, B2 and L share one sort of the witness digits, so their tables share one window shape: the one the
+  // nw witness scalars would get (the MSMs run over nw scalars; the result does not depend on the window)
+  int wwb = wb;
+  if (!wwb) CS_DISPATCH_CURVE(d->curve, { wwb = (int)msm_auto_window(nw, Cfg::FR_BITS); });
+  CS_TRY(cs_bases_upload(ctx, d->curve, CS_G1, d->a_query, d->a_query_len, wwb, &pk->a_query));
+  CS_TRY(cs_bases_upload(ctx, d->curve, CS_G1, d->b_g1_query, d->b_g1_query_len, wwb, &pk->b_g1));
+  CS_TRY(cs_bases_upload(ctx, d->curve, CS_G2, d->b_g2_query, d->b_g2_query_len, wwb, &pk->b_g2));
+  if (nw) CS_TRY(cs_bases_upload(ctx, d->curve, CS_G1, d->l_query, d->l_query_len, wwb, &pk->l_query));
   CS_TRY(cs_bases_upload(ctx, d->curve, CS_G1, d->h_query, n, wb, &pk->h_query));
-  {
-    static int share_env = -1;  // CS_SHARE_B_SORT=0 disables the shared sort (A/B comparison)
-    if (share_env < 0) { const char* e = getenv("CS_SHARE_B_SORT"); share_env = e ? atoi(e) : 1; }
-    if (share_env) CS_TRY(bases_sort_compatible(ctx, pk->b_g1, pk->b_g2, &pk->share_b_sort));
-  }
+  CS_TRY(plan_witness_views(ctx, pk.get()));
   switch (d->curve) {
     case CS_BN254: CS_TRY(build_coset_table<Bn254Cfg>(ctx, pk.get())); break;
 #if defined(CS_ENABLE_BLS12_381)

@@ -44,6 +44,7 @@ static inline size_t fq_limbs64(int curve) { return curve == CS_BN254 ? 4 : 6; }
 static inline size_t point_limbs64(int curve, int group) { return fq_limbs64(curve) * (group == CS_G1 ? 2 : 4); }
 
 constexpr int CS_NSIDE = 5;
+constexpr int CS_WIT_SORT = CS_NSIDE;  // msm_ws slot of the witness sort shared by Groth16's A, B1, B2 and L MSMs
 
 }  // namespace cs
 
@@ -58,7 +59,7 @@ struct cs_ctx {
   cudaEvent_t ev_fork = nullptr;
   cudaEvent_t ev_t0 = nullptr;  // timing event at the last fork, recorded only while MSM profiling is on (cs_msm_timeline_ms)
   cudaEvent_t ev_side[cs::CS_NSIDE] = {};
-  cs::MsmWorkspace msm_ws[cs::CS_NSIDE];
+  cs::MsmWorkspace msm_ws[cs::CS_NSIDE + 1];  // one per side stream, + the shared witness sort (CS_WIT_SORT)
   cs::DevBuf io;  // staging for host-buffer convenience calls
   cs::DevBuf prf_keys;
   cs::DevBuf sc_part, sc_res;  // sumcheck round: per-block partial sums and the 16 results (reused across rounds)
@@ -107,12 +108,13 @@ namespace cs {
 std::atomic<uint64_t>& launch_counter();
 int ctx_fork(cs_ctx* ctx, int nside);
 int ctx_join(cs_ctx* ctx, int nside);
-// sort_slot >= 0: reuse the sorted entries of the MSM last enqueued in that workspace slot (same scalars, same
-// table geometry and infinity pattern -- see msm_enqueue)
+// sort_slot >= 0: the MSM reads the sort last enqueued in that workspace slot over the same scalars -- as it is, or
+// (view) through a filtered view of the shared witness sort; see msm_enqueue
 int msm_enqueue_dyn(cs_ctx* ctx, int slot, cudaStream_t st, const cs_bases* b, size_t offset,
-                    const uint32_t* d_scalars, unsigned sstride, size_t n, int mont, int sort_slot = -1);
-// both base sets sort identically for equal scalars: same length, window shape and infinity mask
-int bases_sort_compatible(cs_ctx* ctx, const cs_bases* a, const cs_bases* b, bool* out);
+                    const uint32_t* d_scalars, unsigned sstride, size_t n, int mont, int sort_slot = -1, bool view = false);
+// Sort of n scalars into workspace `slot` without an infinity mask, entries w * n + i, in the window shape of b
+int msm_sort_shared_dyn(cs_ctx* ctx, int slot, cudaStream_t st, const cs_bases* b, const uint32_t* d_scalars,
+                        unsigned sstride, size_t n, int mont);
 int msm_finish_dyn(cs_ctx* ctx, int slot, const cs_bases* b, uint64_t* out_affine, int* out_inf);
 int ntt_run(cs_ctx* ctx, const cs_domain* d, uint32_t* d_data, unsigned batch, bool inverse_in_to_out,
             const uint32_t* d_post, cudaStream_t st);

@@ -34,8 +34,9 @@ CS_GLOBAL void k_msm_digits(const uint32_t* __restrict__ scalars, uint32_t sstri
   uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
   // bases at infinity (sparse Groth16 B-queries: B_i(tau) = 0 for variables absent from B) contribute
-  // nothing: drop their entries before the sort instead of carrying them through the accumulation
-  if ((infmask[(offset + i) >> 5] >> ((offset + i) & 31)) & 1) {
+  // nothing: drop their entries before the sort instead of carrying them through the accumulation.
+  // infmask = null: keep every entry (the witness sort that several base sets share, filtered per table by k_msm_view_*)
+  if (infmask && ((infmask[(offset + i) >> 5] >> ((offset + i) & 31)) & 1)) {
     for (uint32_t w = 0; w < W; w++) dig[(size_t)w * n + i] = 0;
     return;
   }
@@ -181,6 +182,116 @@ static CS_GLOBAL void k_msm_scatter(const uint32_t* __restrict__ dig, uint32_t n
   if (!b) return;
   uint32_t pos = start[b] + atomicAdd(&cursor[b], 1u);
   sorted[pos] = (w * nbases + offset + i) | (d & MSM_SIGN);
+}
+
+// --------------------------------------------------------------------------- filtered view of a shared sort
+// Groth16's A, B1, B2 and L MSMs take the same witness scalars over different tables.  Their digits are sorted ONCE
+// without an infinity mask (k_msm_digits with infmask = null, entries w * n + i: window w, scalar i); a table with
+// infinity bases, or whose slots are not w * n + i, gets a stream compaction of those entries that drops the entries
+// of its infinite bases and rewrites the rest to its own slots, w * nbases + offset + i.  The compaction keeps the
+// order, so the view is grouped by bucket as the shared entries are, and its bucket counts follow from the kept
+// entries before each shared bucket start: per-block counts and keep bitmaps, no per-entry global atomics.
+constexpr unsigned MSM_VIEW_T = 256;  // entries per block of the view kernels, one per thread
+constexpr unsigned MSM_VIEW_WORDS = MSM_VIEW_T / 32;
+
+CS_D uint32_t popc32(uint32_t x) {
+#if defined(CS_EMU)
+  return (uint32_t)__builtin_popcount(x);
+#else
+  return __popc(x);
+#endif
+}
+// bit l = pred of lane l; every lane of the warp calls it
+CS_D uint32_t warp_bits(bool pred) {
+#if defined(CS_EMU)
+  uint32_t x = pred ? 1u << (threadIdx.x & 31) : 0u;  // distinct bits: the butterfly sum is the OR
+  for (uint32_t d = 16; d > 0; d >>= 1) x += __shfl_xor_sync(0xffffffffu, x, d);
+  return x;
+#else
+  return __ballot_sync(0xffffffffu, pred);
+#endif
+}
+
+// keep[] bit p = shared entry p belongs to a finite base of this table; blk_cnt[block] = kept entries of the block
+static CS_GLOBAL void k_msm_view_flags(const uint32_t* __restrict__ sorted, const uint32_t* __restrict__ src_start,
+                                       uint32_t nb1, uint32_t n, const uint32_t* __restrict__ infmask, uint32_t offset,
+                                       uint32_t* __restrict__ keep, uint32_t* __restrict__ blk_cnt) {
+  __shared__ uint32_t cnt[MSM_VIEW_WORDS];
+  const uint32_t t = threadIdx.x;
+  const uint32_t p = blockIdx.x * MSM_VIEW_T + t;
+  bool k = false;
+  if (p < src_start[nb1]) {  // total shared entries
+    const uint32_t i = (sorted[p] & ~MSM_SIGN) % n;
+    k = !((infmask[(offset + i) >> 5] >> ((offset + i) & 31)) & 1);
+  }
+  const uint32_t bits = warp_bits(k);
+  if ((t & 31) == 0) {
+    keep[(size_t)blockIdx.x * MSM_VIEW_WORDS + (t >> 5)] = bits;
+    cnt[t >> 5] = popc32(bits);
+  }
+  __syncthreads();
+  if (t == 0) {
+    uint32_t c = 0;
+    for (uint32_t w = 0; w < MSM_VIEW_WORDS; w++) c += cnt[w];
+    blk_cnt[blockIdx.x] = c;
+  }
+}
+
+// one block: blk_off = exclusive scan of blk_cnt[0..nblk), blk_off[nblk] = total
+static CS_GLOBAL void k_msm_view_scan(const uint32_t* __restrict__ blk_cnt, uint32_t nblk, uint32_t* __restrict__ blk_off) {
+  __shared__ uint32_t sm[MSM_SCAN_T];
+  const uint32_t t = threadIdx.x, T = blockDim.x;
+  const uint32_t per = (nblk + T - 1) / T;
+  const uint32_t lo = t * per < nblk ? t * per : nblk, hi = lo + per < nblk ? lo + per : nblk;
+  uint32_t s = 0;
+  for (uint32_t b = lo; b < hi; b++) s += blk_cnt[b];
+  sm[t] = s;
+  __syncthreads();
+  for (uint32_t d = 1; d < T; d <<= 1) {
+    const uint32_t v = t >= d ? sm[t - d] : 0;
+    __syncthreads();
+    sm[t] += v;
+    __syncthreads();
+  }
+  uint32_t run = sm[t] - s;
+  for (uint32_t b = lo; b < hi; b++) {
+    const uint32_t c = blk_cnt[b];
+    blk_off[b] = run;
+    run += c;
+  }
+  if (t == T - 1) blk_off[nblk] = run;
+}
+
+// kept entries among shared positions [0, p)
+CS_D uint32_t view_kept_before(uint32_t p, const uint32_t* __restrict__ keep, const uint32_t* __restrict__ blk_off) {
+  const uint32_t blk = p / MSM_VIEW_T;
+  uint32_t r = blk_off[blk];
+  for (uint32_t w = blk * MSM_VIEW_WORDS; w < (p >> 5); w++) r += popc32(keep[w]);
+  if (p & 31) r += popc32(keep[p >> 5] & ((1u << (p & 31)) - 1));
+  return r;
+}
+
+// count[b] of the view: kept entries of shared bucket b
+static CS_GLOBAL void k_msm_view_counts(const uint32_t* __restrict__ src_start, uint32_t nb1, const uint32_t* __restrict__ keep,
+                                        const uint32_t* __restrict__ blk_off, uint32_t* __restrict__ count) {
+  const uint32_t b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b >= nb1) return;
+  count[b] = b ? view_kept_before(src_start[b + 1], keep, blk_off) - view_kept_before(src_start[b], keep, blk_off) : 0;
+}
+
+// kept shared entry p -> position blk_off[block] + rank in the block, rewritten to this table's slot
+static CS_GLOBAL void k_msm_view_scatter(const uint32_t* __restrict__ sorted, uint32_t n, uint32_t nbases, uint32_t offset,
+                                         const uint32_t* __restrict__ keep, const uint32_t* __restrict__ blk_off,
+                                         uint32_t* __restrict__ out) {
+  const uint32_t t = threadIdx.x;
+  const uint32_t* kb = keep + (size_t)blockIdx.x * MSM_VIEW_WORDS;
+  const uint32_t word = kb[t >> 5];
+  if (!((word >> (t & 31)) & 1)) return;
+  uint32_t pos = blk_off[blockIdx.x] + popc32(word & ((1u << (t & 31)) - 1));
+  for (uint32_t k = 0; k < (t >> 5); k++) pos += popc32(kb[k]);
+  const uint32_t e = sorted[blockIdx.x * MSM_VIEW_T + t];
+  const uint32_t v = e & ~MSM_SIGN, w = v / n, i = v - w * n;
+  out[pos] = (w * nbases + offset + i) | (e & MSM_SIGN);
 }
 
 // largest b in [0, nb1) with arr[b] <= s   (arr non-decreasing, arr[0] = 0)
@@ -585,12 +696,139 @@ int msm_accum0_f52(const Affine<F>* table, const uint32_t* sorted, const uint32_
                    const uint32_t* sstart0, uint32_t nb1, uint32_t S, const uint32_t* order, const uint32_t* order_b,
                    Xyzz<F>* part0, uint32_t max_s0, cudaStream_t st);
 
+// Buffer sizes of one MSM over n scalars (W n entries) and the layout of its sort buffers.
+struct MsmSizes {
+  uint32_t nb1, S, ob;
+  size_t nent, max_s0, max_s1, max_s2;
+  MsmSizes(const MsmShape& sh, uint32_t n) {
+    nb1 = sh.B + 1;
+    nent = (size_t)sh.W * n;
+    S = msm_slice(sh);
+    max_s0 = nent / S + nb1;
+    max_s1 = max_s0 / S + nb1;
+    max_s2 = max_s1 / S + nb1;
+    ob = ceil_div(max_s0, MSM_ORDER_BLOCK);
+  }
+  // meta: count[nb1] cursor[nb1] | start[nb1+1] sstart0[nb1+1] sstart1[nb1+1] sstart2[nb1+1] | aux[4 * scan blocks]
+  size_t meta_words() const { return 2 * (size_t)nb1 + 4 * ((size_t)nb1 + 1) + 4 * MSM_SCAN_MAX_BLOCKS; }
+  // slice order: slice_len | slice_bkt | order | order_b (max_s0 each) | block_hist | len_base | chunk_sum
+  size_t order_words() const {
+    return 4 * max_s0 + (size_t)ob * (MSM_SLICE_MAX + 1) + 2 * (MSM_SLICE_MAX + 1) + (size_t)(MSM_SLICE_MAX + 1) * MSM_OFF_CHUNKS;
+  }
+};
+struct MsmSortBufs {
+  uint32_t *count, *cursor, *start, *sstart0, *sstart1, *sstart2, *aux;
+  uint32_t *slice_len, *slice_bkt, *order, *order_b, *block_hist, *len_base, *chunk_sum;
+  MsmSortBufs(const MsmWorkspace& w, const MsmSizes& z) {
+    count = w.meta.as<uint32_t>();
+    cursor = count + z.nb1;
+    start = cursor + z.nb1;
+    sstart0 = start + z.nb1 + 1;
+    sstart1 = sstart0 + z.nb1 + 1;
+    sstart2 = sstart1 + z.nb1 + 1;
+    aux = sstart2 + z.nb1 + 1;
+    slice_len = w.order.as<uint32_t>();
+    slice_bkt = slice_len + z.max_s0;
+    order = slice_bkt + z.max_s0;
+    order_b = order + z.max_s0;
+    block_hist = order_b + z.max_s0;
+    len_base = block_hist + (size_t)z.ob * (MSM_SLICE_MAX + 1);
+    chunk_sum = len_base + 2 * (MSM_SLICE_MAX + 1);
+  }
+};
+
+static inline int msm_check_limits(const MsmShape& sh, uint32_t n, uint32_t nbases) {
+  const size_t nent = (size_t)sh.W * n;
+  if (nent >= (1ull << 31) || (size_t)sh.W * nbases >= (1ull << 31))
+    return fail(-3, "msm: W*n = %zu exceeds 2^31 entries", nent);
+  return 0;
+}
+
+// count[] -> bucket starts and slice offsets (start, sstart0..2)
+static inline int msm_scan(const MsmSortBufs& q, const MsmSizes& z, uint32_t B, cudaStream_t st) {
+  const uint32_t sb = ceil_div(z.nb1, MSM_SCAN_T);
+  if (sb > MSM_SCAN_MAX_BLOCKS) return fail(-3, "msm: %u buckets exceed the scan's limit", B);
+  CS_LAUNCH_SYNC(k_msm_scan1, sb, MSM_SCAN_T, 0, st, q.count, z.nb1, z.S, q.start, q.sstart0, q.sstart1, q.sstart2, q.aux);
+  CS_LAUNCH(k_msm_scan2, sb, MSM_SCAN_T, 0, st, q.count, z.nb1, z.S, q.start, q.sstart0, q.sstart1, q.sstart2, q.aux);
+  return 0;
+}
+
+// Slice order by length; then ws.sorted_ev marks the sorted entries and the order as final.
+static inline int msm_slice_order(MsmWorkspace& ws, const MsmSortBufs& q, const MsmSizes& z, cudaStream_t st) {
+  CS_LAUNCH_SYNC(k_msm_slice_hist, z.ob, MSM_ORDER_BLOCK, 0, st, q.count, q.sstart0, z.nb1, z.S, q.slice_len, q.slice_bkt,
+                 q.block_hist);
+  const uint32_t nt = (MSM_SLICE_MAX + 1) * MSM_OFF_CHUNKS;
+  CS_LAUNCH(k_msm_slice_off1, ceil_div(nt, 128), 128, 0, st, q.block_hist, z.ob, q.chunk_sum);
+  CS_LAUNCH(k_msm_slice_off2, 1, 128, 0, st, q.chunk_sum, q.len_base);
+  CS_LAUNCH(k_msm_slice_off3, ceil_div(nt, 128), 128, 0, st, q.block_hist, z.ob, q.chunk_sum, q.len_base);
+  CS_LAUNCH_SYNC(k_msm_slice_order, z.ob, MSM_ORDER_BLOCK, 0, st, q.slice_len, q.slice_bkt, (uint32_t)z.max_s0, q.sstart0,
+                 z.nb1, q.block_hist, q.len_base, q.order, q.order_b);
+  if (!ws.sorted_ev_made) {
+    CS_CUDA(cudaEventCreateWithFlags(&ws.sorted_ev, cudaEventDisableTiming));
+    ws.sorted_ev_made = true;
+  }
+  CS_CUDA(cudaEventRecord(ws.sorted_ev, st));
+  ws.sorted_once = true;
+  return 0;
+}
+
+// Digits, bucket sort and slice order of n scalars into ws; the entries index table slots w * nbases + offset + i.
+// infmask = null keeps the entries of every base: with nbases = n and offset = 0 that is the shared witness sort,
+// which msm_enqueue reads as it is (a table without infinity bases and slots w * n + i) or through msm_view.
+template <class FrP>
+int msm_sort(MsmWorkspace& ws, const uint32_t* infmask, uint32_t nbases, MsmShape sh, uint32_t offset,
+             const uint32_t* d_scalars, uint32_t sstride, uint32_t n, int mont, cudaStream_t st) {
+  CS_TRY(msm_check_limits(sh, n, nbases));
+  const MsmSizes z(sh, n);
+  CS_TRY(ws.dig.reserve(z.nent * 4));
+  CS_TRY(ws.sorted.reserve(z.nent * 4));
+  CS_TRY(ws.meta.reserve(z.meta_words() * 4));
+  CS_TRY(ws.order.reserve(z.order_words() * 4));
+  const MsmSortBufs q(ws, z);
+  CS_TRY(ws.mark(0, st));
+  CS_CUDA(cudaMemsetAsync(q.count, 0, 2 * (size_t)z.nb1 * 4, st));
+  CS_LAUNCH(k_msm_digits<FrP>, ceil_div(n, 256), 256, 0, st, d_scalars, sstride, n, mont, sh.c, sh.W, infmask, offset,
+            ws.dig.as<uint32_t>(), q.count);
+  CS_TRY(ws.mark(1, st));
+  CS_TRY(msm_scan(q, z, sh.B, st));
+  CS_LAUNCH(k_msm_scatter, dim3(ceil_div(n, 256), sh.W), 256, 0, st, ws.dig.as<uint32_t>(), n, nbases, offset, q.start,
+            q.cursor, ws.sorted.as<uint32_t>());
+  return msm_slice_order(ws, q, z, st);
+}
+
+// This table's entries out of the shared witness sort in src (k_msm_view_*): entries of its infinite bases dropped,
+// the others rewritten to its slots w * nbases + offset + i; then bucket offsets and a slice order of its own.
+static inline int msm_view(MsmWorkspace& ws, const MsmWorkspace& src, const uint32_t* infmask, uint32_t nbases,
+                           MsmShape sh, uint32_t offset, uint32_t n, cudaStream_t st) {
+  const MsmSizes z(sh, n);
+  const uint32_t nblk = ceil_div(z.nent, MSM_VIEW_T);
+  // dig: keep bitmap | blk_cnt[nblk] | blk_off[nblk + 1]
+  CS_TRY(ws.dig.reserve(((size_t)nblk * MSM_VIEW_WORDS + 2 * (size_t)nblk + 1) * 4));
+  CS_TRY(ws.sorted.reserve(z.nent * 4));
+  CS_TRY(ws.meta.reserve(z.meta_words() * 4));
+  CS_TRY(ws.order.reserve(z.order_words() * 4));
+  const MsmSortBufs q(ws, z), s(src, z);
+  uint32_t* keep = ws.dig.as<uint32_t>();
+  uint32_t* blk_cnt = keep + (size_t)nblk * MSM_VIEW_WORDS;
+  uint32_t* blk_off = blk_cnt + nblk;
+  const uint32_t* src_sorted = src.sorted.as<uint32_t>();
+  CS_LAUNCH_SYNC(k_msm_view_flags, nblk, MSM_VIEW_T, 0, st, src_sorted, s.start, z.nb1, n, infmask, offset, keep, blk_cnt);
+  CS_LAUNCH_SYNC(k_msm_view_scan, 1, MSM_SCAN_T, 0, st, blk_cnt, nblk, blk_off);
+  CS_LAUNCH(k_msm_view_counts, ceil_div(z.nb1, 256), 256, 0, st, s.start, z.nb1, keep, blk_off, q.count);
+  CS_LAUNCH(k_msm_view_scatter, nblk, MSM_VIEW_T, 0, st, src_sorted, n, nbases, offset, keep, blk_off,
+            ws.sorted.as<uint32_t>());
+  CS_TRY(msm_scan(q, z, sh.B, st));
+  return msm_slice_order(ws, q, z, st);
+}
+
 // Enqueue one MSM on `st`.  d_scalars: device, n elements of Fr (8 x u32).  The XYZZ result lands in
 // ws.h_result (pinned) after the stream drains.
-// sort_from (optional): another workspace whose MSM was enqueued over the SAME scalars with the same table
-// geometry (nbases, offset, n, window) and the same infinity pattern -- Groth16's B1 / B2 pair.  Its sorted
-// entries and slice order are reused (they index table slots, not points), so this MSM starts at the
-// accumulation; `st` waits for that workspace's sort to finish.
+// sort_from (optional): a workspace holding a sort of the SAME scalars, enqueued earlier; `st` waits for it.
+//  * view = false: its sorted entries and slice order are used as they are (they index table slots, not points), so
+//    this MSM starts at the accumulation.  Table geometry (nbases, offset, n, window) and infinity pattern must
+//    match: Groth16's B2 on B1's entries, or L (no infinity base, slots w * n + i) on the shared witness sort.
+//  * view = true: sort_from holds the shared witness sort (msm_sort without a mask), and this MSM accumulates its
+//    own filtered view of it (msm_view).
 // st_acc (optional): a second, LOWER-priority stream for the accumulation kernel alone.  When several MSMs share the
 // GPU, the block scheduler serves equal-priority grids in launch order, so the short sort / fold / reduce kernels of
 // one MSM queue behind the full-GPU accumulation grids of all the others (measured: folds of an MSM finished at 3 ms
@@ -599,23 +837,11 @@ template <class F, class FrP>
 int msm_enqueue(MsmWorkspace& ws, const Affine<F>* table, const uint32_t* infmask, uint32_t nbases, MsmShape sh,
                 uint32_t offset,
                 const uint32_t* d_scalars, uint32_t sstride, uint32_t n, int mont, cudaStream_t st,
-                MsmWorkspace* sort_from = nullptr, bool table_m260 = false, cudaStream_t st_acc = nullptr) {
-  const uint32_t nb1 = sh.B + 1;
-  const size_t nent = (size_t)sh.W * n;
-  if (nent >= (1ull << 31) || (size_t)sh.W * nbases >= (1ull << 31))
-    return fail(-3, "msm: W*n = %zu exceeds 2^31 entries", nent);
-  const uint32_t S = msm_slice(sh);
-  const size_t max_s0 = nent / S + nb1;
-  const size_t max_s1 = max_s0 / S + nb1;
-  const size_t max_s2 = max_s1 / S + nb1;
-  MsmWorkspace& so = sort_from ? *sort_from : ws;  // owner of the sort buffers
-  // meta: count[nb1] cursor[nb1] | start[nb1+1] sstart0[nb1+1] sstart1[nb1+1] sstart2[nb1+1] | aux[4 * scan blocks]
-  const size_t meta_words = 2 * (size_t)nb1 + 4 * ((size_t)nb1 + 1) + 4 * MSM_SCAN_MAX_BLOCKS;  // + the scan's block totals
-  if (!sort_from) {
-    CS_TRY(ws.dig.reserve(nent * 4));
-    CS_TRY(ws.sorted.reserve(nent * 4));
-    CS_TRY(ws.meta.reserve(meta_words * 4));
-  }
+                MsmWorkspace* sort_from = nullptr, bool view = false, bool table_m260 = false, cudaStream_t st_acc = nullptr) {
+  CS_TRY(msm_check_limits(sh, n, nbases));
+  const MsmSizes z(sh, n);
+  const uint32_t nb1 = z.nb1, S = z.S;
+  const size_t max_s0 = z.max_s0, max_s1 = z.max_s1, max_s2 = z.max_s2;
   CS_TRY(ws.part0.reserve(max_s0 * sizeof(Xyzz<F>)));
   CS_TRY(ws.part1.reserve(max_s1 * sizeof(Xyzz<F>)));
   CS_TRY(ws.part2.reserve(max_s2 * sizeof(Xyzz<F>)));
@@ -626,65 +852,24 @@ int msm_enqueue(MsmWorkspace& ws, const Affine<F>* table, const uint32_t* infmas
   const uint32_t fs_blocks = nseg > 4 * fs_threads ? (nseg + fs_threads - 1) / fs_threads : 1;
   CS_TRY(ws.red.reserve(((size_t)nseg + fs_blocks) * sizeof(Xyzz<F>)));
   CS_TRY(ws.result.reserve(sizeof(Xyzz<F>)));
-  // slice order: slice_len | slice_bkt | order | order_b (max_s0 each) | block_hist | len_base
-  const uint32_t ob = ceil_div(max_s0, MSM_ORDER_BLOCK);
-  const size_t order_words = 4 * max_s0 + (size_t)ob * (MSM_SLICE_MAX + 1) + 2 * (MSM_SLICE_MAX + 1) +
-                             (size_t)(MSM_SLICE_MAX + 1) * MSM_OFF_CHUNKS;
-  if (!sort_from) CS_TRY(ws.order.reserve(order_words * 4));
   if (ws.h_result_cap < sizeof(Xyzz<F>)) {
     if (ws.h_result) cudaFreeHost(ws.h_result);
     CS_CUDA(cudaMallocHost(&ws.h_result, sizeof(Xyzz<F>)));
     ws.h_result_cap = sizeof(Xyzz<F>);
   }
-  uint32_t* slice_len = so.order.as<uint32_t>();
-  uint32_t* slice_bkt = slice_len + max_s0;
-  uint32_t* order = slice_bkt + max_s0;
-  uint32_t* order_b = order + max_s0;
-  uint32_t* block_hist = order_b + max_s0;
-  uint32_t* len_base = block_hist + (size_t)ob * (MSM_SLICE_MAX + 1);
-  uint32_t* chunk_sum = len_base + 2 * (MSM_SLICE_MAX + 1);
-  uint32_t* count = so.meta.as<uint32_t>();
-  uint32_t* cursor = count + nb1;
-  uint32_t* start = cursor + nb1;
-  uint32_t* sstart0 = start + nb1 + 1;
-  uint32_t* sstart1 = sstart0 + nb1 + 1;
-  uint32_t* sstart2 = sstart1 + nb1 + 1;
   if (sort_from) {
     if (!sort_from->sorted_once) return fail(-1, "msm: the workspace to share a sort with has not been enqueued");
     CS_TRY(ws.mark(0, st));
     CS_CUDA(cudaStreamWaitEvent(st, sort_from->sorted_ev, 0));
     CS_TRY(ws.mark(1, st));
+    if (view) CS_TRY(msm_view(ws, *sort_from, infmask, nbases, sh, offset, n, st));
   } else {
-    CS_TRY(ws.mark(0, st));
-    CS_CUDA(cudaMemsetAsync(count, 0, 2 * (size_t)nb1 * 4, st));
-    CS_LAUNCH(k_msm_digits<FrP>, ceil_div(n, 256), 256, 0, st, d_scalars, sstride, n, mont, sh.c, sh.W, infmask, offset,
-              ws.dig.as<uint32_t>(), count);
-    CS_TRY(ws.mark(1, st));
-    {
-      const uint32_t sb = ceil_div(nb1, MSM_SCAN_T);
-      if (sb > MSM_SCAN_MAX_BLOCKS) return fail(-3, "msm: %u buckets exceed the scan's limit", sh.B);
-      uint32_t* aux = sstart2 + nb1 + 1;
-      CS_LAUNCH_SYNC(k_msm_scan1, sb, MSM_SCAN_T, 0, st, count, nb1, S, start, sstart0, sstart1, sstart2, aux);
-      CS_LAUNCH(k_msm_scan2, sb, MSM_SCAN_T, 0, st, count, nb1, S, start, sstart0, sstart1, sstart2, aux);
-    }
-    CS_LAUNCH(k_msm_scatter, dim3(ceil_div(n, 256), sh.W), 256, 0, st, ws.dig.as<uint32_t>(), n, nbases,
-              offset, start, cursor, ws.sorted.as<uint32_t>());
-    CS_LAUNCH_SYNC(k_msm_slice_hist, ob, MSM_ORDER_BLOCK, 0, st, count, sstart0, nb1, S, slice_len, slice_bkt, block_hist);
-    {
-      const uint32_t nt = (MSM_SLICE_MAX + 1) * MSM_OFF_CHUNKS;
-      CS_LAUNCH(k_msm_slice_off1, ceil_div(nt, 128), 128, 0, st, block_hist, ob, chunk_sum);
-      CS_LAUNCH(k_msm_slice_off2, 1, 128, 0, st, chunk_sum, len_base);
-      CS_LAUNCH(k_msm_slice_off3, ceil_div(nt, 128), 128, 0, st, block_hist, ob, chunk_sum, len_base);
-    }
-    CS_LAUNCH_SYNC(k_msm_slice_order, ob, MSM_ORDER_BLOCK, 0, st, slice_len, slice_bkt, (uint32_t)max_s0, sstart0, nb1,
-                   block_hist, len_base, order, order_b);
-    if (!ws.sorted_ev_made) {
-      CS_CUDA(cudaEventCreateWithFlags(&ws.sorted_ev, cudaEventDisableTiming));
-      ws.sorted_ev_made = true;
-    }
-    CS_CUDA(cudaEventRecord(ws.sorted_ev, st));
-    ws.sorted_once = true;
+    CS_TRY(msm_sort<FrP>(ws, infmask, nbases, sh, offset, d_scalars, sstride, n, mont, st));
   }
+  MsmWorkspace& so = sort_from && !view ? *sort_from : ws;  // owner of the sorted entries
+  const MsmSortBufs q(so, z);
+  const uint32_t *count = q.count, *start = q.start, *sstart0 = q.sstart0, *sstart1 = q.sstart1, *sstart2 = q.sstart2;
+  const uint32_t *order = q.order, *order_b = q.order_b;
   CS_TRY(ws.mark(2, st));
   cudaStream_t st_main = st;
   if (st_acc) {

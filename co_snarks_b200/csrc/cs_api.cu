@@ -186,11 +186,17 @@ int cs_memcpy_d2h(cs_ctx* ctx, void* h_dst, const void* d_src, size_t bytes) {
 // ------------------------------------------------------------------------------------------- MSM
 namespace cs {
 
+// widest window an MSM can run: msm_scan takes 2^20 bucket slots, 2^(c-1) buckets plus bucket 0
+constexpr unsigned MSM_MAX_WINDOW = 20;
+static_assert((1u << (MSM_MAX_WINDOW - 1)) + 1 <= MSM_SCAN_MAX_BLOCKS * MSM_SCAN_T, "MSM_MAX_WINDOW exceeds the scan");
+
 template <class Cfg, int G>
 int bases_upload_t(cs_ctx* ctx, const uint64_t* h_points, size_t n, int window_bits, cs_bases* b) {
   typedef typename GroupOf<Cfg, G>::F F;
   unsigned c = window_bits ? (unsigned)window_bits : msm_auto_window(n, Cfg::FR_BITS);
-  if (c < 2 || c > 22) return fail(CS_ERR_ARG, "cs_bases_upload: window_bits %u out of range [2,22]", c);
+  // a window wider than msm_scan takes would build the table and then fail every MSM
+  if (c < 2 || c > MSM_MAX_WINDOW)
+    return fail(CS_ERR_ARG, "cs_bases_upload: window_bits %d out of range [2,%u] (0 = automatic)", window_bits, MSM_MAX_WINDOW);
   b->sh = msm_shape(Cfg::FR_BITS, c);
   b->n = n;
   size_t total = (size_t)b->sh.W * n;

@@ -71,7 +71,9 @@ int cs_memcpy_d2h(cs_ctx* ctx, void* h_dst, const void* d_src, size_t bytes);
  * co-noir/co-noir-common/src/honk_curve.rs:81-83.
  *
  * cs_bases_upload: upload `n` affine points (Montgomery) once per proving key / SRS; the library
- * expands them into the per-window table it keeps resident in HBM.  window_bits = 0 picks a default.
+ * expands them into the per-window table it keeps resident in HBM.  window_bits = 0 picks a default
+ * (at most 16); an explicit window_bits must lie in [2, 20], the widest window the bucket sort takes, and
+ * anything else fails here with CS_ERR_ARG (so does a Groth16 key created with such a window).
  * cs_msm: sum_{i<n} scalars[i] * bases[offset + i]; the reference "chops to the shorter slice"
  * (honk_curve.rs:33-34) -- pass n = min(len).  scalars_montgomery = 1 for `&[Fr]` (msm_unchecked),
  * 0 for canonical `&[BigInt]` (msm_bigint; must be < r).  Result: affine point (Montgomery), all-zero

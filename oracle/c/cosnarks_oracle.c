@@ -195,7 +195,7 @@ static void roots_of_unity(unsigned power, fe* gen, fe* shift) {
 /* ------------------------------------------------------------------ NTT (batch = interleaved components) */
 static unsigned bitrev(unsigned x, unsigned lg) { unsigned r = 0; for (unsigned i = 0; i < lg; i++) r |= ((x >> i) & 1u) << (lg - 1 - i); return r; }
 
-static fe* twiddles(const fe* g, size_t half) {
+static fe* twiddles(const fe* g, size_t half, const fctx* fr) {
   fe* tw = (fe*)malloc((half ? half : 1) * sizeof(fe));
   if (!half) return tw;
   const size_t blk = 4096;
@@ -203,18 +203,18 @@ static fe* twiddles(const fe* g, size_t half) {
   for (long b = 0; b < (long)((half + blk - 1) / blk); b++) {
     size_t lo = (size_t)b * blk, hi = lo + blk < half ? lo + blk : half;
     u64 e[4] = {lo, 0, 0, 0};
-    fe cur; fe_pow(&cur, g, e, &FR);
-    for (size_t k = lo; k < hi; k++) { tw[k] = cur; fe_mul(&cur, &cur, g, &FR); }
+    fe cur; fe_pow(&cur, g, e, fr);
+    for (size_t k = lo; k < hi; k++) { tw[k] = cur; fe_mul(&cur, &cur, g, fr); }
   }
   return tw;
 }
 
-/* natural in -> bit-reversed out (DIF), scaled by 1/n : Domain::ifft_in_to_out */
-static void ifft_in_to_out(fe* a, unsigned lg, unsigned batch, const fe* gen) {
+/* natural in -> bit-reversed out (DIF), scaled by 1/n : Domain::ifft_in_to_out.  fr = the scalar field. */
+static void ifft_in_to_out(fe* a, unsigned lg, unsigned batch, const fe* gen, const fctx* fr) {
   size_t n = (size_t)1 << lg;
   if (lg == 0) return;
-  fe ginv; fe_inv(&ginv, gen, &FR);
-  fe* tw = twiddles(&ginv, n / 2);
+  fe ginv; fe_inv(&ginv, gen, fr);
+  fe* tw = twiddles(&ginv, n / 2, fr);
   for (size_t m = n / 2; m >= 1; m >>= 1) {
     size_t step = (n / 2) / m;
 #pragma omp parallel for schedule(static)
@@ -222,22 +222,22 @@ static void ifft_in_to_out(fe* a, unsigned lg, unsigned batch, const fe* gen) {
       size_t k = ((size_t)bf / m) * 2 * m, j = (size_t)bf % m;
       for (unsigned c = 0; c < batch; c++) {
         fe* x = &a[(k + j) * batch + c]; fe* y = &a[(k + j + m) * batch + c];
-        fe s, d; fe_add(&s, x, y, &FR); fe_sub(&d, x, y, &FR);
-        *x = s; fe_mul(y, &d, &tw[j * step], &FR);
+        fe s, d; fe_add(&s, x, y, fr); fe_sub(&d, x, y, fr);
+        *x = s; fe_mul(y, &d, &tw[j * step], fr);
       }
     }
   }
-  fe ninv; fe_from_u64(&ninv, n, &FR); fe_inv(&ninv, &ninv, &FR);
+  fe ninv; fe_from_u64(&ninv, n, fr); fe_inv(&ninv, &ninv, fr);
 #pragma omp parallel for schedule(static)
-  for (long i = 0; i < (long)(n * batch); i++) fe_mul(&a[i], &a[i], &ninv, &FR);
+  for (long i = 0; i < (long)(n * batch); i++) fe_mul(&a[i], &a[i], &ninv, fr);
   free(tw);
 }
 
 /* bit-reversed in -> natural out (DIT) : Domain::fft_out_to_in */
-static void fft_out_to_in(fe* a, unsigned lg, unsigned batch, const fe* gen) {
+static void fft_out_to_in(fe* a, unsigned lg, unsigned batch, const fe* gen, const fctx* fr) {
   size_t n = (size_t)1 << lg;
   if (lg == 0) return;
-  fe* tw = twiddles(gen, n / 2);
+  fe* tw = twiddles(gen, n / 2, fr);
   for (size_t m = 1; m < n; m <<= 1) {
     size_t step = (n / 2) / m;
 #pragma omp parallel for schedule(static)
@@ -245,8 +245,8 @@ static void fft_out_to_in(fe* a, unsigned lg, unsigned batch, const fe* gen) {
       size_t k = ((size_t)bf / m) * 2 * m, j = (size_t)bf % m;
       for (unsigned c = 0; c < batch; c++) {
         fe* x = &a[(k + j) * batch + c]; fe* y = &a[(k + j + m) * batch + c];
-        fe t, s, d; fe_mul(&t, y, &tw[j * step], &FR);
-        fe_add(&s, x, &t, &FR); fe_sub(&d, x, &t, &FR);
+        fe t, s, d; fe_mul(&t, y, &tw[j * step], fr);
+        fe_add(&s, x, &t, fr); fe_sub(&d, x, &t, fr);
         *x = s; *y = d;
       }
     }
@@ -254,8 +254,20 @@ static void fft_out_to_in(fe* a, unsigned lg, unsigned batch, const fe* gen) {
   free(tw);
 }
 
-int oracle_ifft_in_to_out(u64* data, unsigned lg, unsigned batch, const u64* gen) { ifft_in_to_out((fe*)data, lg, batch, (const fe*)gen); return 0; }
-int oracle_fft_out_to_in(u64* data, unsigned lg, unsigned batch, const u64* gen) { fft_out_to_in((fe*)data, lg, batch, (const fe*)gen); return 0; }
+/* curve: 0 = BN254 Fr, 1 = BLS12-381 Fr (the cs_curve ids of include/cosnarks_gpu.h) */
+static const fctx* fr_of(int curve) { return curve == 0 ? &FR : curve == 1 ? &FR_BLS12_381 : NULL; }
+int oracle_ifft_in_to_out(u64* data, unsigned lg, unsigned batch, const u64* gen, int curve) {
+  const fctx* fr = fr_of(curve);
+  if (!fr) return -1;
+  ifft_in_to_out((fe*)data, lg, batch, (const fe*)gen, fr);
+  return 0;
+}
+int oracle_fft_out_to_in(u64* data, unsigned lg, unsigned batch, const u64* gen, int curve) {
+  const fctx* fr = fr_of(curve);
+  if (!fr) return -1;
+  fft_out_to_in((fe*)data, lg, batch, (const fe*)gen, fr);
+  return 0;
+}
 
 /* ------------------------------------------------------------------ Groth16 (same key descriptor as the C ABI) */
 typedef struct {
@@ -325,7 +337,7 @@ int oracle_witness_map(const key_desc* d, int kind, int party, const u64* pub_, 
   fe gen, shift; roots_of_unity(lg, &gen, &shift);
   /* bit_reversed_coset_table (reduction.rs:45-60) */
   fe* table = (fe*)malloc(n * sizeof(fe));
-  { fe* nat = twiddles(&shift, n);
+  { fe* nat = twiddles(&shift, n, &FR);
 #pragma omp parallel for schedule(static)
     for (long i = 0; i < (long)n; i++) table[bitrev((unsigned)i, lg)] = nat[i];
     free(nat); }
@@ -338,11 +350,11 @@ int oracle_witness_map(const key_desc* d, int kind, int party, const u64* pub_, 
   fe* vecs[3] = {a, b, c};
   unsigned bt[3] = {batch, batch, 1};
   for (int v = 0; v < 3; v++) {
-    ifft_in_to_out(vecs[v], lg, bt[v], &gen);
+    ifft_in_to_out(vecs[v], lg, bt[v], &gen, &FR);
 #pragma omp parallel for schedule(static)
     for (long i = 0; i < (long)n; i++)
       for (unsigned k = 0; k < bt[v]; k++) fe_mul(&vecs[v][(size_t)i * bt[v] + k], &vecs[v][(size_t)i * bt[v] + k], &table[i], &FR);
-    fft_out_to_in(vecs[v], lg, bt[v], &gen);
+    fft_out_to_in(vecs[v], lg, bt[v], &gen, &FR);
   }
   local_mul((fe*)h_out, a, b, batch, kind ? (const fe*)m2 : NULL, c, n);
   free(a); free(b); free(c); free(table);

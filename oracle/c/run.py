@@ -36,13 +36,18 @@ def msm(points_mont, scalars_mont, group=0):
     return out
 
 
-def ifft_in_to_out(data, lg, batch, gen_mont):
-    lib().oracle_ifft_in_to_out(_p(data), C.c_uint(lg), C.c_uint(batch), _p(np.ascontiguousarray(gen_mont)))
+def ifft_in_to_out(data, lg, batch, gen_mont, curve=0):
+    """In place on a contiguous np.uint64 array of Montgomery Fr elements; curve = cs_curve id (0 BN254, 1 BLS12-381)."""
+    assert data.flags.c_contiguous and data.dtype == np.uint64
+    rc = lib().oracle_ifft_in_to_out(_p(data), C.c_uint(lg), C.c_uint(batch), _p(np.ascontiguousarray(gen_mont)), C.c_int(curve))
+    assert rc == 0, "oracle_ifft_in_to_out: unknown curve %d" % curve
     return data
 
 
-def fft_out_to_in(data, lg, batch, gen_mont):
-    lib().oracle_fft_out_to_in(_p(data), C.c_uint(lg), C.c_uint(batch), _p(np.ascontiguousarray(gen_mont)))
+def fft_out_to_in(data, lg, batch, gen_mont, curve=0):
+    assert data.flags.c_contiguous and data.dtype == np.uint64
+    rc = lib().oracle_fft_out_to_in(_p(data), C.c_uint(lg), C.c_uint(batch), _p(np.ascontiguousarray(gen_mont)), C.c_int(curve))
+    assert rc == 0, "oracle_fft_out_to_in: unknown curve %d" % curve
     return data
 
 

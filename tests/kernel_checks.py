@@ -115,6 +115,71 @@ def check_ntt(ctx, log_sizes, seed=3, curve="bn254"):
         dom.free()
 
 
+def rand_fr_limbs(n, seed):
+    """n field elements as limb arrays [n, 4], vectorised: uniform 253-bit values, below r on BN254 and BLS12-381
+    alike, so they serve as canonical values and as Montgomery representations."""
+    rng = np.random.Generator(np.random.PCG64(seed))
+    a = rng.integers(0, 2 ** 63, size=(n, 4), dtype=np.uint64) << np.uint64(1)
+    a |= rng.integers(0, 2, size=(n, 4), dtype=np.uint64)
+    a[:, 3] &= np.uint64((1 << 61) - 1)
+    return a
+
+
+def bitrev_index(lg):
+    """i -> bit reversal of i in lg bits, for i < 2^lg (vectorised)."""
+    i = np.arange(1 << lg, dtype=np.uint64)
+    out = np.zeros_like(i)
+    for b in range(lg):
+        out |= ((i >> np.uint64(b)) & np.uint64(1)) << np.uint64(lg - 1 - b)
+    return out
+
+
+def check_ntt_against_oracle_c(ctx, curve, lg, batch, seed=17):
+    """Every output of the device NTT at 2^lg (batch interleaved components) equals oracle/c's plain radix-2 loop, byte
+    for byte: ifft_in_to_out and fft_out_to_in each on its own input (a round trip would hide an error both directions
+    share, e.g. a twiddle index that the DIF and DIT passes compute alike), the natural-order cs_fft / cs_ifft, and
+    cs_bit_reverse.  ifft_in_to_out stores through the pass's fused 1/n scaling."""
+    from oracle.c import run as OC
+    cv = Conv(curve)
+    n = 1 << lg
+    g, _ = groth16_roots_of_unity(cv.r, lg)
+    gm = cv.fr([g])
+    dom = ctx.domain(cv.id, lg, gm)
+    perm = bitrev_index(lg).astype(np.int64)
+
+    def device(x, run):
+        d = ctx.to_device(x)
+        try:
+            run(d)
+            return ctx.d2h(d, x.shape)
+        finally:
+            ctx.free(d)
+
+    def brev(x):  # bit-reverse the element index of an [n * batch, 4] array, components kept together
+        return np.ascontiguousarray(x.reshape(n, batch, 4)[perm].reshape(n * batch, 4))
+
+    def same(got, exp, what):
+        if not np.array_equal(got, exp):
+            bad = np.nonzero((got != exp).any(axis=1))[0]
+            raise AssertionError("%s %s 2^%d batch %d: %d of %d outputs differ, first at %s"
+                                 % (what, curve, lg, batch, bad.size, n * batch, bad[:4].tolist()))
+
+    lib = ctx.lib
+    x = rand_fr_limbs(n * batch, seed)
+    same(device(x, lambda d: dom.ifft_in_to_out(d, batch)), OC.ifft_in_to_out(x.copy(), lg, batch, gm, cv.id),
+         "ifft_in_to_out")
+    x = rand_fr_limbs(n * batch, seed + 1)
+    same(device(x, lambda d: dom.fft_out_to_in(d, batch)), OC.fft_out_to_in(x.copy(), lg, batch, gm, cv.id),
+         "fft_out_to_in")
+    x = rand_fr_limbs(n * batch, seed + 2)
+    same(device(x, lambda d: dom.fft(d, batch)), OC.fft_out_to_in(brev(x), lg, batch, gm, cv.id), "cs_fft")
+    x = rand_fr_limbs(n * batch, seed + 3)
+    same(device(x, lambda d: dom.ifft(d, batch)), brev(OC.ifft_in_to_out(x.copy(), lg, batch, gm, cv.id)), "cs_ifft")
+    x = rand_fr_limbs(n * batch, seed + 4)
+    same(device(x, lambda d: ctx._check(lib.cs_bit_reverse(ctx.h, cv.id, d, lg, batch))), brev(x), "cs_bit_reverse")
+    dom.free()
+
+
 def _edge_case_inputs(G, gen, n, r, rng):
     pts = [G.mul(gen, rng.randrange(1, r)) for _ in range(n)]
     sc = [rng.randrange(r) for _ in range(n)]
@@ -206,14 +271,19 @@ def check_crs_file_ingest(ctx, tmp_path):
     bases.free()
 
 
-def check_fixed_base_mul(ctx, n=40):
-    cv = Conv("bn254")
+def check_fixed_base_mul(ctx, n=40, curve="bn254"):
+    cv = Conv(curve)
+    C_ = CURVES[curve]
     rng = random.Random(6)
     sc = [rng.randrange(cv.r) for _ in range(n)]
-    sc[0], sc[1] = 0, 1
-    for group, G, gen, to_arr, to_pt in ((0, og1(BN254), BN254.g1, cv.g1, cv.pt1), (1, og2(BN254), BN254.g2, cv.g2, cv.pt2)):
+    edge = [0, 1, cv.r - 1, 2, cv.r - 2, (cv.r - 1) // 2, 1 << 128, (1 << cv.r.bit_length() - 1) - 1]
+    sc[:min(n, len(edge))] = edge[:n]
+    for group, G, gen, to_arr, to_pt in ((0, og1(C_), C_.g1, cv.g1, cv.pt1), (1, og2(C_), C_.g2, cv.g2, cv.pt2)):
+        exp = [G.mul(gen, s) for s in sc]
         out = ctx.fixed_base_mul(cv.id, group, to_arr([gen])[0], cv.fr(sc))
-        assert [to_pt(o) for o in out] == [G.mul(gen, s) for s in sc]
+        assert [to_pt(o) for o in out] == exp, (curve, group, "montgomery")
+        out = ctx.fixed_base_mul(cv.id, group, to_arr([gen])[0], cv.fr_canonical(sc), montgomery=False)
+        assert [to_pt(o) for o in out] == exp, (curve, group, "canonical")
 
 
 def check_plonk_round1_kat(ctx, curve="bn254", name="multiplier2"):

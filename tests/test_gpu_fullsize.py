@@ -204,8 +204,11 @@ def test_groth16_2p20_proof_verifies(gpu_ctx, syn20):
 
 @pytest.mark.parametrize("lg,batch", [(22, 2), (24, 1)])
 def test_ntt_plonk_sizes_roundtrip(gpu_ctx, lg, batch):
-    """co-Plonk domain sizes (BASELINE configs[3]: n = 2^22, extended 4n = 2^24; Rep3 shares = batch 2):
-    3-pass transforms; fft_out_to_in(ifft_in_to_out(x)) == x and the inverse is linear."""
+    """co-Plonk domain sizes (BASELINE configs[3]: n = 2^22, extended 4n = 2^24; Rep3 shares = batch 2): 3-pass
+    transforms.  Every output of each direction, on its own input, of the natural-order transforms and of the bit
+    reversal equals oracle/c's radix-2 loop (tests/test_production_shapes.py has the other pass splits); the round trip
+    fft_out_to_in(ifft_in_to_out(x)) == x is kept as well."""
+    K.check_ntt_against_oracle_c(gpu_ctx, "bn254", lg, batch)
     cv = Conv("bn254")
     n = 1 << lg
     g, _ = groth16_roots_of_unity(cv.r, lg)
@@ -213,10 +216,6 @@ def test_ntt_plonk_sizes_roundtrip(gpu_ctx, lg, batch):
     a = _rand_fr_limbs(n * batch, 7 + lg, cv.r)
     da = gpu_ctx.to_device(a)
     dom.ifft_in_to_out(da, batch)
-    mid = gpu_ctx.d2h(da, (n * batch, 4))
-    assert not (mid == a).all()
-    # constant term check: iNTT output position 0 holds (sum_j x_j) / n for each component
-    x = B.limbs_to_ints(a[0::batch][:4096])  # cheap partial sanity only: exact check below via round trip
     dom.fft_out_to_in(da, batch)
     assert (gpu_ctx.d2h(da, (n * batch, 4)) == a).all()
     gpu_ctx.free(da)

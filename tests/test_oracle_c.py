@@ -27,22 +27,41 @@ def test_c_msm_matches_python_oracle():
         assert to_pt(out) == G.msm(pts, sc)
 
 
-def test_c_ntt_matches_python_oracle():
-    cv = Conv("bn254")
-    rng = random.Random(2)
-    for lg in (1, 4, 9):
+def _c_ntt_matches_python_oracle(curve, log_sizes, seed):
+    cv = Conv(curve)
+    rng = random.Random(seed)
+    for lg in log_sizes:
         n = 1 << lg
         g, _ = groth16_roots_of_unity(cv.r, lg)
         for batch in (1, 2):
             v = [rng.randrange(cv.r) for _ in range(n * batch)]
+            if n * batch >= 4:
+                v[:4] = [0, 1, cv.r - 1, cv.r - 2]
             arr = cv.fr(v)
-            OC.ifft_in_to_out(arr, lg, batch, cv.fr([g]))
+            OC.ifft_in_to_out(arr, lg, batch, cv.fr([g]), curve=cv.id)
             exp = [None] * (n * batch)
             for c in range(batch):
                 exp[c::batch] = ON.ifft_in_to_out(v[c::batch], g, cv.r)
-            assert cv.fr_back(arr) == exp
-            OC.fft_out_to_in(arr, lg, batch, cv.fr([g]))
-            assert cv.fr_back(arr) == v
+            assert cv.fr_back(arr) == exp, (curve, lg, batch)
+            OC.fft_out_to_in(arr, lg, batch, cv.fr([g]), curve=cv.id)
+            assert cv.fr_back(arr) == v, (curve, lg, batch)
+            # the forward transform on its own input (a round trip cannot show an error both directions share)
+            w = [rng.randrange(cv.r) for _ in range(n * batch)]
+            arr = cv.fr(w)
+            OC.fft_out_to_in(arr, lg, batch, cv.fr([g]), curve=cv.id)
+            for c in range(batch):
+                nat = ON.bit_reverse_perm(w[c::batch])
+                assert cv.fr_back(arr[c::batch]) == [sum(x * pow(g, i * j, cv.r) for j, x in enumerate(nat)) % cv.r
+                                                     for i in range(n)], (curve, lg, batch)
+
+
+def test_c_ntt_matches_python_oracle():
+    _c_ntt_matches_python_oracle("bn254", (1, 4, 9), 2)
+
+
+def test_c_ntt_bls12_381_matches_python_oracle():
+    """oracle/c's BLS12-381 Fr context (4 x 64-bit limbs, 255-bit r) against the Python oracle and the definition."""
+    _c_ntt_matches_python_oracle("bls12_381", (1, 2, 5, 8), 3)
 
 
 @pytest.mark.parametrize("name", ["multiplier2", "poseidon"])

@@ -177,19 +177,20 @@ int oracle_msm_g2(const u64* points, const u64* scalars_mont, size_t sstride_wor
 }
 
 /* ------------------------------------------------------------------ roots of unity (groth16.rs:60-100) */
-static void roots_of_unity(unsigned power, fe* gen, fe* shift) {
+/* fr = the scalar field, s = its two-adicity (r - 1 = 2^s * trace, trace odd) */
+static void roots_of_unity(unsigned power, fe* gen, fe* shift, const fctx* fr, unsigned s) {
   u64 half[4], trace[4];
-  memcpy(half, FR.p, 32); half[0] -= 1; memcpy(trace, half, 32);
+  memcpy(half, fr->p, 32); half[0] -= 1; memcpy(trace, half, 32);
   for (int i = 0; i < 4; i++) half[i] = (half[i] >> 1) | (i < 3 ? half[i + 1] << 63 : 0);
-  for (int s = 0; s < 28; s++) for (int i = 0; i < 4; i++) trace[i] = (trace[i] >> 1) | (i < 3 ? trace[i + 1] << 63 : 0);
-  fe zero, minus_one, q, t; memset(&zero, 0, sizeof(zero)); fe_sub(&minus_one, &zero, &FR.one, &FR);
+  for (unsigned k = 0; k < s; k++) for (int i = 0; i < 4; i++) trace[i] = (trace[i] >> 1) | (i < 3 ? trace[i + 1] << 63 : 0);
+  fe zero, minus_one, q, t; memset(&zero, 0, sizeof(zero)); fe_sub(&minus_one, &zero, &fr->one, fr);
   u64 qv = 1;
-  for (;;) { fe_from_u64(&q, qv, &FR); fe_pow(&t, &q, half, &FR); if (fe_eq(&t, &minus_one)) break; qv++; }
-  fe z; fe_pow(&z, &q, trace, &FR);
+  for (;;) { fe_from_u64(&q, qv, fr); fe_pow(&t, &q, half, fr); if (fe_eq(&t, &minus_one)) break; qv++; }
+  fe z; fe_pow(&z, &q, trace, fr);
   *gen = z;
-  for (unsigned k = 0; k < 28 - power; k++) fe_mul(gen, gen, gen, &FR);
-  if (power == 28) fe_mul(shift, &q, &q, &FR);
-  else { *shift = z; for (unsigned k = 0; k + 1 < 28 - power; k++) fe_mul(shift, shift, shift, &FR); }
+  for (unsigned k = 0; k < s - power; k++) fe_mul(gen, gen, gen, fr);
+  if (power == s) fe_mul(shift, &q, &q, fr);
+  else { *shift = z; for (unsigned k = 0; k + 1 < s - power; k++) fe_mul(shift, shift, shift, fr); }
 }
 
 /* ------------------------------------------------------------------ NTT (batch = interleaved components) */
@@ -287,7 +288,7 @@ typedef struct {
 
 /* evaluate_constraint (reduction.rs:196-210; mpc/plain.rs:29-43, mpc/rep3.rs:31-49) */
 static void spmv(fe* out, const uint32_t* rp, const uint32_t* col, const fe* cf, const fe* pub, size_t ni,
-                 const fe* wit, unsigned batch, int pub_comp, size_t nrows, size_t npubrows, size_t n) {
+                 const fe* wit, unsigned batch, int pub_comp, size_t nrows, size_t npubrows, size_t n, const fctx* fr) {
 #pragma omp parallel for schedule(static)
   for (long r = 0; r < (long)n; r++) {
     fe acc[2]; memset(acc, 0, sizeof(acc));
@@ -295,10 +296,10 @@ static void spmv(fe* out, const uint32_t* rp, const uint32_t* col, const fe* cf,
       for (uint32_t k = rp[r]; k < rp[r + 1]; k++) {
         fe t;
         if (col[k] < ni) {
-          if (pub_comp >= 0) { fe_mul(&t, &cf[k], &pub[col[k]], &FR); fe_add(&acc[pub_comp], &acc[pub_comp], &t, &FR); }
+          if (pub_comp >= 0) { fe_mul(&t, &cf[k], &pub[col[k]], fr); fe_add(&acc[pub_comp], &acc[pub_comp], &t, fr); }
         } else {
           size_t wi = (size_t)(col[k] - ni) * batch;
-          for (unsigned c = 0; c < batch; c++) { fe_mul(&t, &cf[k], &wit[wi + c], &FR); fe_add(&acc[c], &acc[c], &t, &FR); }
+          for (unsigned c = 0; c < batch; c++) { fe_mul(&t, &cf[k], &wit[wi + c], fr); fe_add(&acc[c], &acc[c], &t, fr); }
         }
       }
     } else if ((size_t)r < nrows + npubrows) {
@@ -309,54 +310,58 @@ static void spmv(fe* out, const uint32_t* rp, const uint32_t* col, const fe* cf,
 }
 
 /* local_mul_vec (+ optional mask, optional subtraction) -- rep3/arithmetic.rs:132-146, ops.rs:69-76 */
-static void local_mul(fe* out, const fe* a, const fe* b, unsigned batch, const fe* mask, const fe* sub, size_t n) {
+static void local_mul(fe* out, const fe* a, const fe* b, unsigned batch, const fe* mask, const fe* sub, size_t n, const fctx* fr) {
 #pragma omp parallel for schedule(static)
   for (long i = 0; i < (long)n; i++) {
     fe z;
-    if (batch == 1) fe_mul(&z, &a[i], &b[i], &FR);
+    if (batch == 1) fe_mul(&z, &a[i], &b[i], fr);
     else {
       fe t1, t2, t3;
-      fe_mul(&t1, &a[2 * i], &b[2 * i], &FR); fe_mul(&t2, &a[2 * i], &b[2 * i + 1], &FR); fe_mul(&t3, &a[2 * i + 1], &b[2 * i], &FR);
-      fe_add(&z, &t1, &t2, &FR); fe_add(&z, &z, &t3, &FR);
+      fe_mul(&t1, &a[2 * i], &b[2 * i], fr); fe_mul(&t2, &a[2 * i], &b[2 * i + 1], fr); fe_mul(&t3, &a[2 * i + 1], &b[2 * i], fr);
+      fe_add(&z, &t1, &t2, fr); fe_add(&z, &z, &t3, fr);
     }
-    if (mask) fe_add(&z, &z, &mask[i], &FR);
-    if (sub) fe_sub(&z, &z, &sub[i], &FR);
+    if (mask) fe_add(&z, &z, &mask[i], fr);
+    if (sub) fe_sub(&z, &z, &sub[i], fr);
     out[i] = z;
   }
 }
 
-/* CircomReduction::witness_map_from_matrices.  kind 0 = plain, 1 = rep3 (party 0..2).  h: n elements. */
+/* CircomReduction::witness_map_from_matrices.  kind 0 = plain, 1 = rep3 (party 0..2).  h: n elements.
+ * The scalar field, two-adicity and roots follow d->curve (0 BN254: s = 28, 1 BLS12-381: s = 32). */
 int oracle_witness_map(const key_desc* d, int kind, int party, const u64* pub_, const u64* wit_, const u64* m1,
                        const u64* m2, u64* h_out) {
   const size_t nc = d->num_constraints, ni = d->num_instance_variables;
+  const fctx* fr = fr_of(d->curve);
+  if (!fr) return -1;
+  const unsigned two_adicity = d->curve == 0 ? 28 : 32;
   size_t n = 1; unsigned lg = 0;
   while (n < nc + ni) { n <<= 1; lg++; }
-  if (lg > 28) return -1;
+  if (lg > two_adicity) return -1;
   const unsigned batch = kind ? 2 : 1;
   const int pub_comp = kind ? (party == 0 ? 0 : (party == 1 ? 1 : -1)) : 0;
-  fe gen, shift; roots_of_unity(lg, &gen, &shift);
+  fe gen, shift; roots_of_unity(lg, &gen, &shift, fr, two_adicity);
   /* bit_reversed_coset_table (reduction.rs:45-60) */
   fe* table = (fe*)malloc(n * sizeof(fe));
-  { fe* nat = twiddles(&shift, n, &FR);
+  { fe* nat = twiddles(&shift, n, fr);
 #pragma omp parallel for schedule(static)
     for (long i = 0; i < (long)n; i++) table[bitrev((unsigned)i, lg)] = nat[i];
     free(nat); }
   fe* a = (fe*)malloc(n * batch * sizeof(fe));
   fe* b = (fe*)malloc(n * batch * sizeof(fe));
   fe* c = (fe*)malloc(n * sizeof(fe));
-  spmv(a, d->a_row_ptr, d->a_col, (const fe*)d->a_coeff, (const fe*)pub_, ni, (const fe*)wit_, batch, pub_comp, nc, ni, n);
-  spmv(b, d->b_row_ptr, d->b_col, (const fe*)d->b_coeff, (const fe*)pub_, ni, (const fe*)wit_, batch, pub_comp, nc, 0, n);
-  local_mul(c, a, b, batch, kind ? (const fe*)m1 : NULL, NULL, n);
+  spmv(a, d->a_row_ptr, d->a_col, (const fe*)d->a_coeff, (const fe*)pub_, ni, (const fe*)wit_, batch, pub_comp, nc, ni, n, fr);
+  spmv(b, d->b_row_ptr, d->b_col, (const fe*)d->b_coeff, (const fe*)pub_, ni, (const fe*)wit_, batch, pub_comp, nc, 0, n, fr);
+  local_mul(c, a, b, batch, kind ? (const fe*)m1 : NULL, NULL, n, fr);
   fe* vecs[3] = {a, b, c};
   unsigned bt[3] = {batch, batch, 1};
   for (int v = 0; v < 3; v++) {
-    ifft_in_to_out(vecs[v], lg, bt[v], &gen, &FR);
+    ifft_in_to_out(vecs[v], lg, bt[v], &gen, fr);
 #pragma omp parallel for schedule(static)
     for (long i = 0; i < (long)n; i++)
-      for (unsigned k = 0; k < bt[v]; k++) fe_mul(&vecs[v][(size_t)i * bt[v] + k], &vecs[v][(size_t)i * bt[v] + k], &table[i], &FR);
-    fft_out_to_in(vecs[v], lg, bt[v], &gen, &FR);
+      for (unsigned k = 0; k < bt[v]; k++) fe_mul(&vecs[v][(size_t)i * bt[v] + k], &vecs[v][(size_t)i * bt[v] + k], &table[i], fr);
+    fft_out_to_in(vecs[v], lg, bt[v], &gen, fr);
   }
-  local_mul((fe*)h_out, a, b, batch, kind ? (const fe*)m2 : NULL, c, n);
+  local_mul((fe*)h_out, a, b, batch, kind ? (const fe*)m2 : NULL, c, n, fr);
   free(a); free(b); free(c); free(table);
   return 0;
 }
@@ -365,6 +370,7 @@ int oracle_witness_map(const key_desc* d, int kind, int party, const u64* pub_, 
 int oracle_groth16_prove_plain(const key_desc* d, const u64* pub_, const u64* wit_, const u64* r_m, const u64* s_m,
                                u64* out_a, u64* out_b, u64* out_c) {
   const size_t nc = d->num_constraints, ni = d->num_instance_variables, nw = d->num_witness_variables;
+  if (d->curve != 0) return -1;  /* G1/G2 here are BN254's (4-limb Fq) */
   size_t n = 1; while (n < nc + ni) n <<= 1;
   fe* h = (fe*)malloc(n * sizeof(fe));
   if (oracle_witness_map(d, 0, 0, pub_, wit_, NULL, NULL, (u64*)h)) { free(h); return -1; }

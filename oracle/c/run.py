@@ -51,12 +51,13 @@ def fft_out_to_in(data, lg, batch, gen_mont, curve=0):
     return data
 
 
-def key_desc(matrices_csr, points):
-    """Same descriptor as co_snarks_b200.binding.KeyDesc (include/cosnarks_gpu.h: cs_groth16_key_desc)."""
+def key_desc(matrices_csr, points, curve=0):
+    """Same descriptor as co_snarks_b200.binding.KeyDesc (include/cosnarks_gpu.h: cs_groth16_key_desc).  curve = cs_curve
+    id: the witness map follows it (BN254 or BLS12-381 Fr); prove_plain takes BN254 keys only."""
     from co_snarks_b200.binding import KeyDesc, u32p, u64p  # type definition only
     d = KeyDesc()
     keep = []
-    d.curve = 0
+    d.curve = curve
     d.num_constraints = matrices_csr["num_constraints"]
     d.num_instance_variables = matrices_csr["num_instance_variables"]
     d.num_witness_variables = matrices_csr["num_witness_variables"]
@@ -83,7 +84,7 @@ def witness_map(desc, kind, party, pub, wit, m1=None, m2=None):
         n <<= 1
     out = np.zeros((n, 4), dtype=np.uint64)
     rc = lib().oracle_witness_map(C.byref(desc), kind, party, _p(pub), _p(wit), _p(m1), _p(m2), _p(out))
-    assert rc == 0
+    assert rc == 0, "oracle_witness_map: unknown curve %d or domain beyond its two-adicity" % desc.curve
     return out
 
 

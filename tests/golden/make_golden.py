@@ -279,3 +279,4 @@ if __name__ == "__main__":
     plonk_full_fixture("poseidon", True)
     plonk_full_fixture("multiplier2", False, "bls12_381")
     groth16_fixture("multiplier2", [(0, 0), (11, 13)], False, "bls12_381")
+    groth16_fixture("poseidon", [(123456789, 987654321)], True, "bls12_381")

@@ -17,6 +17,15 @@ from oracle.fields import BN254, CURVES, groth16_roots_of_unity
 from oracle.pairing_bn254 import groth16_verify
 
 
+def groth16_verifier(curve):
+    """The pairing check of `curve`'s Groth16 verifier (oracle.pairing_*.groth16_verify)."""
+    if curve == "bls12_381":
+        from oracle.pairing_bls12_381 import groth16_verify as verify
+        return verify
+    assert curve == "bn254", curve
+    return groth16_verify
+
+
 def check_field_ops(ctx, n=257, seed=1, curve="bn254"):
     cv = Conv(curve)
     r = cv.r
@@ -79,12 +88,17 @@ def check_share_kernels(ctx, n=300, seed=2):
         ctx.free(d)
 
 
-def check_roots(ctx):
-    cv = Conv("bn254")
-    for power in (0, 1, 2, 8, 20, 27, 28):
+def check_roots(ctx, curve="bn254"):
+    """cs_groth16_roots_of_unity == groth16.rs:60-100 at every power up to the field's two-adicity (28 on BN254, 32 on
+    BLS12-381; at the two-adicity itself the coset shift is qnr^2), and a power above it is refused."""
+    cv = Conv(curve)
+    s = cv.c.two_adicity
+    for power in sorted({0, 1, 2, 8, 20, 27, 28, s - 1, s}):
         gen, shift = ctx.roots_of_unity(cv.id, power)
         eg, es = groth16_roots_of_unity(cv.r, power)
-        assert cv.fr_back(gen) == [eg] and cv.fr_back(shift) == [es], power
+        assert cv.fr_back(gen) == [eg] and cv.fr_back(shift) == [es], (curve, power)
+    with pytest.raises(B.CsError, match="Polynomial Degree too large"):
+        ctx.roots_of_unity(cv.id, s + 1)
 
 
 def check_ntt(ctx, log_sizes, seed=3, curve="bn254"):
@@ -316,9 +330,7 @@ def check_groth16_fixture(ctx, name, rep3=True, window_bits=0, curve="bn254"):
     cv = Conv(curve)
     r = cv.r
     z, m, w, g = golden_groth16(name, curve)
-    verify = groth16_verify
-    if curve == "bls12_381":
-        from oracle.pairing_bls12_381 import groth16_verify as verify
+    verify = groth16_verifier(curve)
     ni = m["num_instance_variables"]
     pk = make_key(ctx, cv, z, m, window_bits)
     assert pk.domain_size() == g["domain_size"]
@@ -364,11 +376,11 @@ def check_groth16_rep3_local(ctx, pk, cv, z, m, w, h_exp, vk, public, seed=5):
         sh = cv.fr([x for ab in wsh[i] for x in ab])
         hh = pk.witness_map(pub, sh, B.CS_REP3, i, cv.fr(m1[i]), cv.fr(m2[i]))
         h_i = cv.fr_back(hh)
-        assert h_i == OG.witness_map_rep3(i, m, w[:ni], wsh[i], m1[i], m2[i], r, 28)
+        assert h_i == OG.witness_map_rep3(i, m, w[:ni], wsh[i], m1[i], m2[i], r, cv.c.two_adicity)
         h_tot = [(x + y) % r for x, y in zip(h_tot, h_i)]
         loc.append(pk.rep3_local(i, pub, sh, cv.fr(m1[i]), cv.fr(m2[i]), cv.fr(list(rsh[i][0])), cv.fr(list(ssh[i][0]))))
     assert h_tot == h_exp
-    G1, G2 = og1(BN254), og2(BN254)
+    G1, G2 = og1(cv.c), og2(cv.c)
     # open_half_point(A)
     A = None
     for i in range(3):
@@ -390,7 +402,7 @@ def check_groth16_rep3_local(ctx, pk, cv, z, m, w, h_exp, vk, public, seed=5):
     r_tot = sum(x[0][0] for x in rsh) % r
     s_tot = sum(x[0][0] for x in ssh) % r
     assert (A, Bp, C) == OG.prove_plain(z, m, w, r_tot, s_tot)
-    assert groth16_verify(vk, public, (A, Bp, C))
+    assert groth16_verifier(cv.c.name)(vk, public, (A, Bp, C))
 
 
 def check_msm_rep3_shares(ctx, n=200, seed=8):
@@ -406,18 +418,18 @@ def check_msm_rep3_shares(ctx, n=200, seed=8):
     bases.free()
 
 
-def check_groth16_shamir_local(ctx, name="multiplier2", seed=9):
+def check_groth16_shamir_local(ctx, name="multiplier2", seed=9, curve="bn254"):
     """ShamirCoGroth16 (t = 1, n = 3, the only valid 3-party setting: shamir.rs:41-43): the three
     parties' local phases on degree-1 shares, opened by Lagrange interpolation at 0 with weights
     (3, -3, 1) as degree-2 sharings (shamir/pointshare.rs:102-111), give the plain proof for
     r = r(0), s = s(0)."""
-    cv = Conv("bn254")
+    cv = Conv(curve)
     r = cv.r
     rng = random.Random(seed)
-    z, m, w, g = golden_groth16(name)
+    z, m, w, g = golden_groth16(name, curve)
     ni = m["num_instance_variables"]
     pk = make_key(ctx, cv, z, m)
-    G1, G2 = og1(BN254), og2(BN254)
+    G1, G2 = og1(cv.c), og2(cv.c)
 
     def shamir(v):  # degree-1 polynomial, party i evaluates at i + 1
         a = rng.randrange(r)
@@ -446,6 +458,7 @@ def check_groth16_shamir_local(ctx, name="multiplier2", seed=9):
         gc.append(c)
     C = open_(gc, G1)
     assert (A, Bp, C) == OG.prove_plain(z, m, w, r0, s0)
+    assert groth16_verifier(curve)(OG.vk_from_zkey(z), [ih(x) for x in g["public"]], (A, Bp, C))
     pk.free()
 
 
@@ -865,32 +878,47 @@ def check_shamir_degree_reduce(ctx, n=64, seed=12):
         ctx.free(d)
 
 
-def check_zkey_ingest(ctx, tmp_path, name="multiplier2"):
+def check_zkey_ingest(ctx, tmp_path, name="multiplier2", curve="bn254"):
     """cs_groth16_pk_from_zkey + cs_wtns_read (co-circom.rs:1005-1016): a snarkjs-format key/witness pair goes
     file -> device and proves to the golden proof bytes; the writer's output is also parsed by the oracle's
-    reader, and the reference's own files are ingested too."""
+    reader, and the reference's own files are ingested too.  The test writer emits 32-byte fields, so on BLS12-381
+    (48-byte Fq) only the reference's own files are ingested; there the proof also verifies under the reference's
+    snarkjs verification_key.json and the key's public inputs equal its public.json."""
+    import json
     import os
     import zkey_writer
     from oracle import formats as OF
     from oracle.formats import proof_to_json
-    cv = Conv("bn254")
-    z, m, w, g = golden_groth16(name)
-    zp, wp = os.path.join(str(tmp_path), name + ".zkey"), os.path.join(str(tmp_path), name + ".wtns")
-    zkey_writer.write_zkey(zp, z, m)
-    zkey_writer.write_wtns(wp, cv.r, w)
-    z2 = OF.read_groth16_zkey(zp)  # the test writer agrees with the oracle's reader
-    assert z2["a_query"] == z["a_query"] and OF.zkey_matrices(z2)["a"] == m["a"]
-    ref = "test_vectors/Groth16/bn254/%s/" % name
-    files = [(zp, wp), (reference_file(ref + "circuit.zkey", tmp_path), reference_file(ref + "witness.wtns", tmp_path))]
+    cv = Conv(curve)
+    z, m, w, g = golden_groth16(name, curve)
+    ref = "test_vectors/Groth16/%s/%s/" % (curve, name)
+    files = [(reference_file(ref + "circuit.zkey", tmp_path), reference_file(ref + "witness.wtns", tmp_path))]
+    if curve == "bn254":
+        zp, wp = os.path.join(str(tmp_path), name + ".zkey"), os.path.join(str(tmp_path), name + ".wtns")
+        zkey_writer.write_zkey(zp, z, m)
+        zkey_writer.write_wtns(wp, cv.r, w)
+        z2 = OF.read_groth16_zkey(zp)  # the test writer agrees with the oracle's reader
+        assert z2["a_query"] == z["a_query"] and OF.zkey_matrices(z2)["a"] == m["a"]
+        files.insert(0, (zp, wp))
+    vk = None
+    if curve == "bls12_381":
+        vk = OF.read_vk_json(reference_file(ref + "verification_key.json", tmp_path))
+        public = [int(x) for x in json.load(open(reference_file(ref + "public.json", tmp_path)))]
+        assert public == [ih(x) for x in g["public"]]
     for zf, wf in files:
-        pk = B.Groth16Key.from_zkey(ctx, zf)
+        pk = B.Groth16Key.from_zkey(ctx, zf, cv.id)
         assert pk.domain_size() == g["domain_size"] and pk.ni == m["num_instance_variables"]
-        wit = B.read_wtns(ctx.lib, wf)
+        wit = B.read_wtns(ctx.lib, wf, cv.id)
         assert cv.fr_back(wit) == w
+        if vk is not None:
+            assert cv.fr_back(wit[1:pk.ni]) == public
         for pr in g["oracle_proofs"]:
             A, Bp, Cp = pk.prove_plain(np.ascontiguousarray(wit[:pk.ni]), np.ascontiguousarray(wit[pk.ni:]),
                                        cv.fr([ih(pr["r"])]), cv.fr([ih(pr["s"])]))
-            assert proof_to_json(cv.pt1(A), cv.pt2(Bp), cv.pt1(Cp)) == pr["json"]
+            proof = (cv.pt1(A), cv.pt2(Bp), cv.pt1(Cp))
+            assert proof_to_json(*proof, "bn128" if curve == "bn254" else "bls12381") == pr["json"]
+            if vk is not None:
+                assert groth16_verifier(curve)(vk, public, proof)
         pk.free()
     # error behaviour
     bad = os.path.join(str(tmp_path), "bad.zkey")

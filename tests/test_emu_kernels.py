@@ -18,6 +18,7 @@ def test_emu_share_kernels(emu_ctx):
 
 def test_emu_roots(emu_ctx):
     K.check_roots(emu_ctx)
+    K.check_roots(emu_ctx, "bls12_381")
 
 
 def test_emu_ntt(emu_ctx):
@@ -152,7 +153,22 @@ def test_crs_file_ingest(emu_ctx, tmp_path):
 def test_emu_groth16_bls12_381(emu_ctx):
     """Groth16 on BLS12-381 (6-limb Fq, 255-bit Fr): witness map and proof bytes == oracle on the reference's
     bls12_381/multiplier2 fixture, proof accepted by the BLS12-381 pairing check under the snarkjs key."""
-    K.check_groth16_fixture(emu_ctx, "multiplier2", rep3=False, curve="bls12_381")
+    K.check_groth16_fixture(emu_ctx, "multiplier2", curve="bls12_381")
+
+
+def test_emu_groth16_bls12_381_poseidon(emu_ctx):
+    """The reference's bls12_381/poseidon circuit: witness map == golden h, proof bytes == the oracle's, and the Rep3
+    local phases of three parties open to the plain proof."""
+    K.check_groth16_fixture(emu_ctx, "poseidon", curve="bls12_381")
+
+
+@pytest.mark.parametrize("name", ["multiplier2", "poseidon"])
+def test_emu_groth16_shamir_local_bls12_381(emu_ctx, name):
+    K.check_groth16_shamir_local(emu_ctx, name, curve="bls12_381")
+
+
+def test_emu_zkey_ingest_bls12_381(emu_ctx, tmp_path):
+    K.check_zkey_ingest(emu_ctx, tmp_path, "poseidon", curve="bls12_381")
 
 
 def test_emu_rep3_batch_vm_ops(emu_ctx):

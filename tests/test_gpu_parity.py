@@ -17,6 +17,7 @@ def test_share_kernels(gpu_ctx):
 
 def test_roots(gpu_ctx):
     K.check_roots(gpu_ctx)
+    K.check_roots(gpu_ctx, "bls12_381")
 
 
 def test_ntt_small(gpu_ctx):
@@ -158,7 +159,22 @@ def test_groth16_bls12_381(gpu_ctx):
     """Groth16 on the BLS12-381 instantiation (6-limb Fq, 255-bit Fr) on the GPU: witness map + five MSMs + assembly on
     the reference's bls12_381/multiplier2 fixture; proof bytes == oracle, accepted by the BLS12-381 pairing check
     under the snarkjs verification key (the acceptance criterion of co-groth16/src/lib.rs:93-119)."""
-    K.check_groth16_fixture(gpu_ctx, "multiplier2", rep3=False, curve="bls12_381")
+    K.check_groth16_fixture(gpu_ctx, "multiplier2", curve="bls12_381")
+
+
+def test_groth16_bls12_381_poseidon(gpu_ctx):
+    """The reference's bls12_381/poseidon circuit on the GPU: witness map == golden h, proof bytes == the oracle's,
+    accepted under the snarkjs key; the Rep3 local phases of three parties open to the plain proof."""
+    K.check_groth16_fixture(gpu_ctx, "poseidon", curve="bls12_381")
+
+
+@pytest.mark.parametrize("name", ["multiplier2", "poseidon"])
+def test_groth16_shamir_local_bls12_381(gpu_ctx, name):
+    K.check_groth16_shamir_local(gpu_ctx, name, curve="bls12_381")
+
+
+def test_zkey_ingest_bls12_381(gpu_ctx, tmp_path):
+    K.check_zkey_ingest(gpu_ctx, tmp_path, "poseidon", curve="bls12_381")
 
 
 def test_msm_fp64_pipe_accumulation_subprocess():

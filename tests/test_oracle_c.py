@@ -94,6 +94,33 @@ def test_c_groth16_equals_golden_proof(name):
 
 
 @pytest.mark.parametrize("name", ["multiplier2", "poseidon"])
+def test_c_witness_map_bls12_381_equals_golden(name):
+    """oracle_witness_map on a BLS12-381 key (key_desc curve 1): its Fr, two-adicity 32 and that field's roots and
+    coset shift give the golden h of the reference's BLS12-381 fixture, plain and as Rep3 shares."""
+    cv = Conv("bls12_381")
+    z, m, w, g = golden_groth16(name, "bls12_381")
+    ni = m["num_instance_variables"]
+    mats = dict(num_constraints=m["num_constraints"], num_instance_variables=ni,
+                num_witness_variables=m["num_witness_variables"], a=cv.csr(m["a"]), b=cv.csr(m["b"]))
+    desc, keep = OC.key_desc(mats, {k: np.zeros((1, 24), dtype=np.uint64) for k in (
+        "alpha_g1", "beta_g1", "beta_g2", "delta_g1", "delta_g2", "a_query", "b_g1_query", "b_g2_query", "l_query",
+        "h_query")}, curve=cv.id)
+    pub, wit = cv.fr(w[:ni]), cv.fr(w[ni:])
+    assert cv.fr_back(OC.witness_map(desc, 0, 0, pub, wit)) == [ih(x) for x in g["h"]]
+    rng = random.Random(6)
+    wsh = OG.share_rep3(w[ni:], cv.r, rng)
+    n = len(g["h"])
+    m1 = [rng.randrange(cv.r) for _ in range(n)]
+    m2 = [rng.randrange(cv.r) for _ in range(n)]
+    for party in range(3):
+        got = cv.fr_back(OC.witness_map(desc, 1, party, pub, cv.fr([x for ab in wsh[party] for x in ab]), cv.fr(m1), cv.fr(m2)))
+        assert got == OG.witness_map_rep3(party, m, w[:ni], wsh[party], m1, m2, cv.r, 32)
+    # a BLS12-381 key cannot go through the BN254-only prover
+    with pytest.raises(AssertionError):
+        OC.prove_plain(desc, pub, wit, cv.fr([1]), cv.fr([2]))
+
+
+@pytest.mark.parametrize("name", ["multiplier2", "poseidon"])
 def test_c_plonk_prover_matches_python_oracle_and_kats(name):
     """oracle/c/plonk.inc (the CPU baseline of the Plonk row) == oracle/plonk.py == the reference's known answers."""
     from helpers import golden_plonk, plonk_key_arrays, plonk_proof_from_device

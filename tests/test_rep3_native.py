@@ -51,9 +51,8 @@ def _check_against_oracle(name, results, curve="bn254"):
     r_tot = sum(x[4][0] for x in res) % r
     s_tot = sum(x[4][2] for x in res) % r
     assert proofs[0] == OG.prove_plain(z, m, w, r_tot, s_tot), "opened Rep3 proof != plain proof for (sum r, sum s)"
-    if curve == "bn254":
-        from oracle.pairing_bn254 import groth16_verify
-        assert groth16_verify(OG.vk_from_zkey(z), [ih(x) for x in g["public"]], proofs[0])
+    from kernel_checks import groth16_verifier
+    assert groth16_verifier(curve)(OG.vk_from_zkey(z), [ih(x) for x in g["public"]], proofs[0])
     return proofs[0]
 
 
@@ -136,6 +135,17 @@ def test_rep3_native_three_threads_emu():
 
 def test_rep3_native_two_gpus_per_party_emu():
     _run_threads(_emu_factory(), "multiplier2", two_gpus=True)
+
+
+@pytest.mark.parametrize("name", ["multiplier2", "poseidon"])
+def test_rep3_native_three_threads_bls12_381_emu(name):
+    """cs_groth16_rep3_prove on BLS12-381 keys: host scalar multiplications on 6-limb Fq, the EC mask and both network
+    legs; the opened proof equals the oracle's plain proof and verifies under the BLS12-381 pairing."""
+    _run_threads(_emu_factory(), name, curve="bls12_381")
+
+
+def test_rep3_native_two_gpus_per_party_bls12_381_emu():
+    _run_threads(_emu_factory(), "multiplier2", two_gpus=True, curve="bls12_381")
 
 
 def test_net_mailbox_large_message_emu():
@@ -340,3 +350,23 @@ def test_rep3_native_two_gpus_per_party_threads_gpu():
         k[0] += 1
         return B.Context((k[0] - 1) % nd)
     _run_threads(mk, "poseidon", two_gpus=True)
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("name", ["multiplier2", "poseidon"])
+def test_rep3_native_three_threads_bls12_381_gpu(name):
+    from co_snarks_b200 import binding as B
+    _run_threads(lambda: B.Context(0), name, curve="bls12_381")
+
+
+@pytest.mark.gpu
+def test_rep3_native_two_gpus_per_party_threads_bls12_381_gpu():
+    from co_snarks_b200 import binding as B
+    import torch
+    nd = torch.cuda.device_count()
+    k = [0]
+
+    def mk():
+        k[0] += 1
+        return B.Context((k[0] - 1) % nd)
+    _run_threads(mk, "poseidon", two_gpus=True, curve="bls12_381")

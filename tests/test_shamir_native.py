@@ -120,14 +120,14 @@ def _degree_reduce_vectors(mk, n, t, length):
         c.close()
 
 
-def _shamir_groth16(mk, name, n=3, t=1, bridge=False):
-    from co_snarks_b200 import binding as B
+def _shamir_groth16(mk, name, n=3, t=1, bridge=False, curve="bn254"):
     from helpers import Conv, golden_groth16, ih, make_key
+    from kernel_checks import groth16_verifier
     from oracle import groth16 as OG
-    from oracle.pairing_bn254 import groth16_verify
-    cv = Conv("bn254")
+    groth16_verify = groth16_verifier(curve)
+    cv = Conv(curve)
     r = cv.r
-    z, m, w, g = golden_groth16(name)
+    z, m, w, g = golden_groth16(name, curve)
     ni = m["num_instance_variables"]
     pub = cv.fr(w[:ni])
     ctxs = [mk() for _ in range(n)]
@@ -199,6 +199,16 @@ def test_groth16_prove_with_shamir_bridge_emu():
     _shamir_groth16(_emu_factory(), "multiplier2", bridge=True)
 
 
+@pytest.mark.parametrize("name", ["multiplier2", "poseidon"])
+def test_shamir_co_groth16_native_bls12_381_emu(name):
+    _shamir_groth16(_emu_factory(), name, curve="bls12_381")
+
+
+@pytest.mark.parametrize("name", ["multiplier2", "poseidon"])
+def test_groth16_prove_with_shamir_bridge_bls12_381_emu(name):
+    _shamir_groth16(_emu_factory(), name, bridge=True, curve="bls12_381")
+
+
 def test_shamir_state_rejects_large_threshold_emu():
     from co_snarks_b200 import binding as B
     mk = _emu_factory()
@@ -225,3 +235,17 @@ def test_shamir_co_groth16_native_gpu():
 def test_groth16_prove_with_shamir_bridge_gpu():
     from co_snarks_b200 import binding as B
     _shamir_groth16(lambda: B.Context(0), "poseidon", bridge=True)
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("name", ["multiplier2", "poseidon"])
+def test_shamir_co_groth16_native_bls12_381_gpu(name):
+    from co_snarks_b200 import binding as B
+    _shamir_groth16(lambda: B.Context(0), name, curve="bls12_381")
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("name", ["multiplier2", "poseidon"])
+def test_groth16_prove_with_shamir_bridge_bls12_381_gpu(name):
+    from co_snarks_b200 import binding as B
+    _shamir_groth16(lambda: B.Context(0), name, bridge=True, curve="bls12_381")

@@ -95,6 +95,7 @@ SIGNATURES = {
     "cs_shamir_degree_reduce_many": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
     "cs_shamir_degree_reduce_point": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p]),
     "cs_shamir_open_half_point": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
+    "cs_shamir_double_sharings": (C.c_int, [C.c_void_p] * 3 + [C.c_size_t, C.c_void_p, C.c_void_p]),
     "cs_groth16_shamir_prove": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int] + [C.c_void_p] * 6),
     "cs_groth16_prove_with_shamir_bridge": (C.c_int, [C.c_void_p] * 10),
     "cs_share_rep3_device": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_size_t, C.c_char_p, C.c_void_p, C.c_void_p, C.c_void_p]),
@@ -190,6 +191,12 @@ SIGNATURES = {
     "cs_plonk_rep3_step": (C.c_int, [C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
     "cs_plonk_rep3_prf_words": (C.c_uint64, [C.c_void_p]),
     "cs_plonk_rep3_connect_io": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p]),
+    "cs_plonk_shamir_create": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_void_p)]),
+    "cs_plonk_shamir_free": (None, [C.c_void_p]),
+    "cs_plonk_shamir_prove": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t] + [C.c_void_p] * 4),
+    "cs_plonk_shamir_pairs": (C.c_size_t, [C.c_void_p]),
+    "cs_plonk_shamir_pair_ms": (C.c_double, [C.c_void_p]),
+    "cs_plonk_shamir_device_bytes": (C.c_size_t, [C.c_void_p]),
     "cs_plonk_rep3_prove": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p,
                                       C.c_void_p, C.c_void_p]),
     "cs_chacha_keystream": (C.c_int, [C.c_void_p, C.c_char_p, C.c_uint64, C.c_uint, C.c_uint, C.c_void_p]),
@@ -699,6 +706,48 @@ class PlonkRep3Session:
     def free(self):
         if self.h:
             self.ctx.lib.cs_plonk_rep3_free(self.h)
+            self.h = None
+
+
+class PlonkShamirSession:
+    """One party's Shamir(n, t) co-Plonk prover (cs_plonk_shamir): ShamirCoPlonk::prove inside the library."""
+
+    def __init__(self, ctx, pk, num_parties, threshold, party):
+        self.ctx, self.pk, self.party = ctx, pk, party
+        h = C.c_void_p()
+        ctx._check(ctx.lib.cs_plonk_shamir_create(ctx.h, pk.h, num_parties, threshold, party, C.byref(h)))
+        self.h = h
+
+    def prove(self, net, public_inputs, witness_shares, blinder_shares=None):
+        """-> (points [9, 2 fq]: A B C Z T1 T2 T3 Wxi Wxiw, evals [6, 4]: a b c s1 s2 zw, this party's 11 blinder
+        shares [11, 4]); witness / blinder shares are degree-t Shamir shares (Montgomery), blinders drawn if None."""
+        pub = np.ascontiguousarray(public_inputs, dtype=np.uint64).reshape(-1, 4)
+        wit = np.ascontiguousarray(witness_shares, dtype=np.uint64).reshape(-1, 4)
+        bl = None
+        if blinder_shares is not None:
+            bl = np.ascontiguousarray(blinder_shares, dtype=np.uint64).reshape(-1, 4)
+            assert bl.shape[0] == 11
+        pts = np.zeros((9, 2 * self.pk.fq), dtype=np.uint64)
+        evs = np.zeros((6, 4), dtype=np.uint64)
+        bout = np.zeros((11, 4), dtype=np.uint64)
+        self.ctx._check(self.ctx.lib.cs_plonk_shamir_prove(self.h, net.h, _ptr(pub), pub.shape[0], _ptr(wit) if wit.shape[0] else None,
+                                                           wit.shape[0], _ptr(bl), _ptr(pts), _ptr(evs), _ptr(bout)))
+        return pts, evs, bout
+
+    def pairs(self):
+        """double sharings the last proof consumed (58 domain_size + 2, + 11 when the blinders were drawn)"""
+        return int(self.ctx.lib.cs_plonk_shamir_pairs(self.h))
+
+    def pair_ms(self):
+        return float(self.ctx.lib.cs_plonk_shamir_pair_ms(self.h))
+
+    def device_bytes(self):
+        """device memory this party's session and Shamir state hold (its high-water mark after a proof)"""
+        return int(self.ctx.lib.cs_plonk_shamir_device_bytes(self.h))
+
+    def free(self):
+        if self.h:
+            self.ctx.lib.cs_plonk_shamir_free(self.h)
             self.h = None
 
 

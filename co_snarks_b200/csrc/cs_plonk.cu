@@ -7,10 +7,12 @@
 // consumes exactly that order spread at stride 4 (bitrev_4n(j) = 4 bitrev_n(j) for j < n), so only the
 // coefficient vectors that are committed / evaluated are permuted back.
 #include <algorithm>
+#include <chrono>
 #include "cs_lib.cuh"
 #include "cs_net.h"
 #include "cs_plonk.cuh"
 #include "cs_plonk_rep3.cuh"
+#include "cs_shamir.cuh"
 
 using namespace cs;
 
@@ -295,6 +297,70 @@ int divide_by_linear(cs_ctx* ctx, H* pk, uint32_t* p, uint32_t len, const host::
   return 0;
 }
 
+// Z_H weights of the blinding terms on the four cosets of the extended domain (mul4vec_post, round3.rs:20-108), from
+// the 4th root of unity roots[2] (types.rs:105)
+template <class Cfg>
+int quotient_consts(int curve, PlonkConsts& K) {
+  typedef host::HFp<typename Cfg::FrP> HR;
+  uint64_t g4[HR::N], unused[HR::N];
+  CS_TRY(cs_groth16_roots_of_unity((cs_curve)curve, 2, g4, unused));
+  HR w4, one = HR::one(), two = one + one, zero = HR::zero();
+  memcpy(w4.l, g4, sizeof(w4.l));
+  HR z1[4] = {zero, w4 - one, zero - two, zero - one - w4};
+  HR z2[4] = {zero, zero - two * w4, two + two, two * w4};
+  HR z3[4] = {zero, two + two * w4, zero - (two + two + two + two), two - two * w4};
+  for (int i = 0; i < 4; i++) { put(K.z1[i], z1[i]); put(K.z2[i], z2[i]); put(K.z3[i], z3[i]); }
+  return 0;
+}
+
+// Round 5's scalars (round5.rs:284-340; calculate_lagrange_evaluations / calculate_pi, lib.rs:181-219): the weights of
+// the linearisation polynomial's terms.  pub: the key's n_public public inputs without the leading slot; ev: the opened
+// eval_a eval_b eval_c eval_s1 eval_s2 eval_zw; beta, gamma, alpha, alpha2, k1, k2 are read from K.
+template <class Cfg>
+int lin_weights(const cs_plonk_pk* pk, const uint64_t* pub, const PlonkConsts& K, const host::HFp<typename Cfg::FrP>& xi,
+                const host::HFp<typename Cfg::FrP>& v0, const host::HFp<typename Cfg::FrP>* ev, PlonkLinW& W) {
+  typedef host::HFp<typename Cfg::FrP> HR;
+  auto ld = [](const uint32_t* w) { HR x; memcpy(x.l, w, sizeof(x.l)); return x; };
+  const HR beta = ld(K.beta), gamma = ld(K.gamma), alpha = ld(K.alpha), alpha2 = ld(K.alpha2), k1 = ld(K.k1), k2 = ld(K.k2);
+  const HR ea = ev[0], eb = ev[1], ec = ev[2], es1 = ev[3], es2 = ev[4], ezw = ev[5];
+  HR v[5];
+  v[0] = v0;
+  for (int i = 1; i < 5; i++) v[i] = v[i - 1] * v[0];
+  HR w_n;
+  memcpy(w_n.l, pk->dom->group_gen.data(), sizeof(w_n.l));
+  HR xin = xi;
+  for (unsigned q = 0; q < pk->log_n; q++) xin = xin.sqr();
+  const HR zh = xin - HR::one();
+  const HR nn = HR::from_u64(pk->n);
+  std::vector<HR> ls(pk->nlag);
+  {
+    HR wi = HR::one();
+    for (uint32_t i = 0; i < pk->nlag; i++) {
+      HR dnm = nn * (xi - wi);
+      if (dnm.is_zero()) return fail(CS_ERR_ARG, "plonk: xi hit the evaluation domain");
+      ls[i] = wi * zh * dnm.inverse();
+      wi = wi * w_n;
+    }
+  }
+  HR eval_pi = HR::zero();
+  for (uint32_t i = 0; i < pk->n_public && i < pk->nlag; i++) {
+    HR val;
+    memcpy(val.l, pub + (size_t)i * HR::N, sizeof(val.l));
+    eval_pi = eval_pi - ls[i] * val;
+  }
+  const HR betaxi = beta * xi;
+  const HR e2 = (ea + betaxi + gamma) * (eb + betaxi * k1 + gamma) * (ec + betaxi * k2 + gamma) * alpha;
+  const HR e3 = (ea + beta * es1 + gamma) * (eb + beta * es2 + gamma) * ezw * alpha;
+  const HR e4 = alpha2 * ls[0];
+  const HR r0 = eval_pi - e3 * (ec + gamma) - e4;
+  memset(&W, 0, sizeof(W));
+  put(W.ab, ea * eb); put(W.ea, ea); put(W.eb, eb); put(W.ec, ec); put(W.e3beta, e3 * beta); put(W.e24, e2 + e4);
+  put(W.zh, zh); put(W.xin, xin); put(W.xin2, xin.sqr());
+  for (int i = 0; i < 5; i++) put(W.v[i], v[i]);
+  put(W.c0, r0 - v[0] * ea - v[1] * eb - v[2] * ec - v[3] * es1 - v[4] * es2);
+  return 0;
+}
+
 template <class Cfg>
 int plonk_prove_plain_t(cs_ctx* ctx, cs_plonk_pk* pk, const uint64_t* h_pub, const uint64_t* h_wit, const uint64_t* h_blind,
                         uint64_t* out_points, uint64_t* out_evals) {
@@ -386,17 +452,7 @@ int plonk_prove_plain_t(cs_ctx* ctx, cs_plonk_pk* pk, const uint64_t* h_pub, con
   const HR alpha = tr.get_challenge();
   const HR alpha2 = alpha.sqr();
   put(K.alpha, alpha); put(K.alpha2, alpha2);
-  {
-    uint64_t g4[HR::N], unused[HR::N];
-    CS_TRY(cs_groth16_roots_of_unity((cs_curve)pk->curve, 2, g4, unused));  // roots[2] (types.rs:105)
-    HR w4, one = HR::one(), two = one + one;
-    memcpy(w4.l, g4, sizeof(w4.l));
-    HR zero = HR::zero();
-    HR z1[4] = {zero, w4 - one, zero - two, zero - one - w4};
-    HR z2[4] = {zero, zero - two * w4, two + two, two * w4};
-    HR z3[4] = {zero, two + two * w4, zero - (two + two + two + two), two - two * w4};
-    for (int i = 0; i < 4; i++) { put(K.z1[i], z1[i]); put(K.z2[i], z2[i]); put(K.z3[i], z3[i]); }
-  }
+  CS_TRY(quotient_consts<Cfg>(pk->curve, K));
   PlonkQuotIn qi;
   qi.a = ev[0]; qi.b = ev[1]; qi.c = ev[2]; qi.z = ev[3];
   qi.qm = pk->q_evals[0].as<uint32_t>(); qi.ql = pk->q_evals[1].as<uint32_t>(); qi.qr = pk->q_evals[2].as<uint32_t>();
@@ -434,41 +490,9 @@ int plonk_prove_plain_t(cs_ctx* ctx, cs_plonk_pk* pk, const uint64_t* h_pub, con
   tr = Transcript<Cfg>();
   tr.add_scalar(xi); tr.add_scalar(ea); tr.add_scalar(eb); tr.add_scalar(ec);
   tr.add_scalar(es1); tr.add_scalar(es2); tr.add_scalar(ezw);
-  HR v[5];
-  v[0] = tr.get_challenge();
-  for (int i = 1; i < 5; i++) v[i] = v[i - 1] * v[0];
-  // calculate_lagrange_evaluations / calculate_pi (lib.rs:181-219)
-  HR xin = xi;
-  for (unsigned s = 0; s < pk->log_n; s++) xin = xin.sqr();
-  const HR zh = xin - HR::one();
-  const HR nn = HR::from_u64(n);
-  std::vector<HR> ls(pk->nlag);
-  {
-    HR wi = HR::one();
-    for (uint32_t i = 0; i < pk->nlag; i++) {
-      HR dnm = nn * (xi - wi);
-      if (dnm.is_zero()) return fail(CS_ERR_ARG, "plonk: xi hit the evaluation domain");
-      ls[i] = wi * zh * dnm.inverse();
-      wi = wi * w_n;
-    }
-  }
-  HR eval_pi = HR::zero();
-  for (uint32_t i = 0; i < npub && i < pk->nlag; i++) {
-    HR val;
-    memcpy(val.l, h_pub + (size_t)(i + 1) * HR::N, sizeof(val.l));
-    eval_pi = eval_pi - ls[i] * val;
-  }
-  const HR betaxi = beta * xi;
-  const HR e2 = (ea + betaxi + gamma) * (eb + betaxi * k1 + gamma) * (ec + betaxi * k2 + gamma) * alpha;
-  const HR e3 = (ea + beta * es1 + gamma) * (eb + beta * es2 + gamma) * ezw * alpha;
-  const HR e4 = alpha2 * ls[0];
-  const HR r0 = eval_pi - e3 * (ec + gamma) - e4;
+  const HR evs5[6] = {ea, eb, ec, es1, es2, ezw};
   PlonkLinW W;
-  memset(&W, 0, sizeof(W));
-  put(W.ab, ea * eb); put(W.ea, ea); put(W.eb, eb); put(W.ec, ec); put(W.e3beta, e3 * beta); put(W.e24, e2 + e4);
-  put(W.zh, zh); put(W.xin, xin); put(W.xin2, xin.sqr());
-  for (int i = 0; i < 5; i++) put(W.v[i], v[i]);
-  put(W.c0, r0 - v[0] * ea - v[1] * eb - v[2] * ec - v[3] * es1 - v[4] * es2);
+  CS_TRY(lin_weights<Cfg>(pk, h_pub + HR::N, K, xi, tr.get_challenge(), evs5, W));
   PlonkLinIn li;
   li.qm = pk->q_coeffs[0].as<uint32_t>(); li.ql = pk->q_coeffs[1].as<uint32_t>(); li.qr = pk->q_coeffs[2].as<uint32_t>();
   li.qo = pk->q_coeffs[3].as<uint32_t>(); li.qc = pk->q_coeffs[4].as<uint32_t>();
@@ -608,8 +632,9 @@ int r3_round1_t(cs_plonk_rep3* s, const uint64_t* h_pub, const uint64_t* h_wit_s
 }
 
 // elementwise inverse of `cnt` public values at `v` (device) into `out`; scratch: 2 cnt elements at `scr`
-template <class Cfg>
-int r3_batch_inverse(cs_plonk_rep3* s, const uint32_t* v, uint32_t cnt, uint32_t* scr, uint32_t* out) {
+// H: a session with `ctx`, `totals` and `small` (Rep3 or Shamir)
+template <class Cfg, class H>
+int r3_batch_inverse(H* s, const uint32_t* v, uint32_t cnt, uint32_t* scr, uint32_t* out) {
   typedef typename Cfg::FrP FrP;
   typedef host::HFp<FrP> HR;
   cs_ctx* ctx = s->ctx;
@@ -621,7 +646,7 @@ int r3_batch_inverse(cs_plonk_rep3* s, const uint32_t* v, uint32_t cnt, uint32_t
   CS_CUDA(cudaStreamSynchronize(ctx->stream));
   if (total.is_zero()) return fail(CS_ERR_ARG, "Cannot invert zero");  // rep3 inv_vec, arithmetic.rs:245-262
   HR it = total.inverse();
-  uint32_t* d_it = s->small.as<uint32_t>() + 128 * FrP::N;
+  uint32_t* d_it = s->small.template as<uint32_t>() + 128 * FrP::N;
   CS_CUDA(cudaMemcpyAsync(d_it, it.l, sizeof(it.l), cudaMemcpyHostToDevice, ctx->stream));
   CS_LAUNCH(k_batch_inverse<FrP>, ceil_div(cnt, 128), 128, 0, ctx->stream, pre, suf, d_it, cnt, out);
   CS_CUDA(cudaStreamSynchronize(ctx->stream));  // `it` is a stack variable
@@ -646,13 +671,13 @@ int r3_step_t(cs_plonk_rep3* s, int step, const uint64_t* h_in, uint64_t* h_out)
     case CS_PLONK_R3_ROUND2_A: {  // in: beta, gamma
       memcpy(s->K.beta, h_in, 32);
       memcpy(s->K.gamma, h_in + HR::N, 32);
-      CS_LAUNCH(k_r3_round2_a<FrP>, gb, 128, 0, st, r3_round2_in<Cfg>(s), s->K, n, s->party, s->prf, s->ctr, r3_slot(s, 0),
+      CS_LAUNCH(k_r3_round2_a<Rep3Pol<FrP>>, gb, 128, 0, st, r3_round2_in<Cfg>(s), s->K, n, s->party, s->prf, s->ctr, r3_slot(s, 0),
                 r3_slot(s, 1), r3_peer(s, 0), r3_peer(s, 1));
       s->ctr += 2 * (uint64_t)n;
       break;
     }
     case CS_PLONK_R3_ROUND2_B: {
-      CS_LAUNCH(k_r3_round2_b<FrP>, gb, 128, 0, st, r3_round2_in<Cfg>(s), s->K, n, s->party, s->prf, s->ctr, r3_slot(s, 0),
+      CS_LAUNCH(k_r3_round2_b<Rep3Pol<FrP>>, gb, 128, 0, st, r3_round2_in<Cfg>(s), s->K, n, s->party, s->prf, s->ctr, r3_slot(s, 0),
                 r3_slot(s, 1), r3_slot(s, 2), r3_slot(s, 3), r3_peer(s, 2), r3_peer(s, 3));
       s->ctr += 2 * (uint64_t)n;
       break;
@@ -660,7 +685,7 @@ int r3_step_t(cs_plonk_rep3* s, int step, const uint64_t* h_in, uint64_t* h_out)
     case CS_PLONK_R3_ROUND2_C: {  // out: g (n) | q (n + 1), additive
       s->rbase = s->ctr;
       s->ctr += 2 * (3 * (uint64_t)n + 2);  // 3n + 2 random shares s, r, s' of 64 bytes each (two element slots)
-      CS_LAUNCH(k_r3_round2_c<FrP>, ceil_div(n + 1, 128), 128, 0, st, r3_slot(s, 3), n, s->prf, s->rbase, s->ctr, addv,
+      CS_LAUNCH(k_r3_round2_c<Rep3Pol<FrP>>, ceil_div(n + 1, 128), 128, 0, st, r3_slot(s, 3), n, s->prf, s->rbase, s->ctr, addv,
                 addv + (size_t)n * NW);
       s->ctr += 2 * (uint64_t)n + 1;
       if (h_out) CS_CUDA(cudaMemcpyAsync(h_out, addv, (size_t)(2 * n + 1) * 32, cudaMemcpyDeviceToHost, st));
@@ -672,18 +697,18 @@ int r3_step_t(cs_plonk_rep3* s, int step, const uint64_t* h_in, uint64_t* h_out)
       if (h_in) CS_CUDA(cudaMemcpyAsync(opened, h_in, (size_t)(2 * n + 1) * 32, cudaMemcpyHostToDevice, st));
       CS_TRY(r3_batch_inverse<Cfg>(s, opened, n, pscr, ginv));
       CS_TRY(r3_batch_inverse<Cfg>(s, opened + (size_t)n * NW, n + 1, pscr, qinv));
-      CS_LAUNCH(k_r3_round2_d<FrP>, gb, 128, 0, st, r3_slot(s, 2), ginv, qinv, n, s->prf, s->rbase, s->ctr, r3_slot(s, 4),
+      CS_LAUNCH(k_r3_round2_d<Rep3Pol<FrP>>, gb, 128, 0, st, r3_slot(s, 2), ginv, qinv, n, s->prf, s->rbase, s->ctr, r3_slot(s, 4),
                 r3_slot(s, 5), r3_peer(s, 4), r3_peer(s, 5));
       s->ctr += 2 * (uint64_t)n;
       break;
     }
     case CS_PLONK_R3_ROUND2_E: {
-      CS_LAUNCH(k_r3_round2_e<FrP>, gb, 128, 0, st, r3_slot(s, 4), n, s->prf, s->rbase, s->ctr, r3_slot(s, 6), r3_peer(s, 6));
+      CS_LAUNCH(k_r3_round2_e<Rep3Pol<FrP>>, gb, 128, 0, st, r3_slot(s, 4), n, s->prf, s->rbase, s->ctr, r3_slot(s, 6), r3_peer(s, 6));
       s->ctr += n;
       break;
     }
     case CS_PLONK_R3_ROUND2_F: {  // out: y (n), additive
-      CS_LAUNCH(k_r3_round2_f<FrP>, gb, 128, 0, st, r3_slot(s, 6), qinv, n, s->prf, s->rbase, s->ctr, addv);
+      CS_LAUNCH(k_r3_round2_f<Rep3Pol<FrP>>, gb, 128, 0, st, r3_slot(s, 6), qinv, n, s->prf, s->rbase, s->ctr, addv);
       s->ctr += n;
       if (h_out) CS_CUDA(cudaMemcpyAsync(h_out, addv, (size_t)n * 32, cudaMemcpyDeviceToHost, st));
       CS_CUDA(cudaStreamSynchronize(st));
@@ -695,7 +720,7 @@ int r3_step_t(cs_plonk_rep3* s, int step, const uint64_t* h_in, uint64_t* h_out)
       else CS_CUDA(cudaMemcpyAsync(y, pscr + (size_t)(4 * n + 4) * NW, (size_t)n * 32, cudaMemcpyDeviceToDevice, st));
       CS_TRY((scan<FrP, 0>(ctx, s, y, y, n, 0)));
       uint32_t* ps = s->polysh[3].as<uint32_t>();
-      CS_LAUNCH(k_r3_round2_g<FrP>, gb, 128, 0, st, y, r3_slot(s, 5), n, ps);
+      CS_LAUNCH(k_r3_round2_g<Rep3Pol<FrP>>, gb, 128, 0, st, y, r3_slot(s, 5), n, ps);
       CS_TRY(interpolate_and_extend<Cfg>(ctx, pk, ps, s->ev[3].as<uint32_t>(), 2));
       HR bsh[6];
       for (int i = 0; i < 3; i++) { memcpy(bsh[2 * i].l, s->B.b[6 + i].v[0], 32); memcpy(bsh[2 * i + 1].l, s->B.b[6 + i].v[1], 32); }
@@ -709,18 +734,11 @@ int r3_step_t(cs_plonk_rep3* s, int step, const uint64_t* h_in, uint64_t* h_out)
       memcpy(alpha.l, h_in, 32);
       put(s->K.alpha, alpha);
       put(s->K.alpha2, alpha.sqr());
-      uint64_t g4[HR::N], unused[HR::N];
-      CS_TRY(cs_groth16_roots_of_unity((cs_curve)pk->curve, 2, g4, unused));
-      HR w4, one = HR::one(), two = one + one, zero = HR::zero();
-      memcpy(w4.l, g4, sizeof(w4.l));
-      HR z1[4] = {zero, w4 - one, zero - two, zero - one - w4};
-      HR z2[4] = {zero, zero - two * w4, two + two, two * w4};
-      HR z3[4] = {zero, two + two * w4, zero - (two + two + two + two), two - two * w4};
-      for (int i = 0; i < 4; i++) { put(s->K.z1[i], z1[i]); put(s->K.z2[i], z2[i]); put(s->K.z3[i], z3[i]); }
+      CS_TRY(quotient_consts<Cfg>(pk->curve, s->K));
       R3QuotIn qi;
       qi.a = s->ev[0].as<uint32_t>(); qi.b = s->ev[1].as<uint32_t>(); qi.c = s->ev[2].as<uint32_t>(); qi.z = s->ev[3].as<uint32_t>();
       qi.tw4 = pk->dom4->tw_fwd.template as<uint32_t>();
-      CS_LAUNCH(k_r3_quot_l1<FrP>, ceil_div(n4, 64), 64, 0, st, qi, s->B, n, s->prf, s->ctr, s->arena.as<uint32_t>(), s->next_arena,
+      CS_LAUNCH(k_r3_quot_l1<Rep3Pol<FrP>>, ceil_div(n4, 64), 64, 0, st, qi, s->B, n, s->prf, s->ctr, s->arena.as<uint32_t>(), s->next_arena,
                 s->slot_words);
       s->ctr += 12 * (uint64_t)n4;
       break;
@@ -735,7 +753,7 @@ int r3_step_t(cs_plonk_rep3* s, int step, const uint64_t* h_in, uint64_t* h_out)
       E.s1 = pk->s_evals[0].as<uint32_t>(); E.s2 = pk->s_evals[1].as<uint32_t>(); E.s3 = pk->s_evals[2].as<uint32_t>();
       E.lagrange = pk->lagrange.as<uint32_t>(); E.buf_a = s->buf[0].as<uint32_t>();
       uint32_t *t = s->t.as<uint32_t>(), *tz = s->tz.as<uint32_t>();
-      CS_LAUNCH(k_r3_quot_l2<FrP>, ceil_div(n4, 64), 64, 0, st, qi, s->B, E, n, pk->nlag, s->K, s->party, s->prf, s->ctr,
+      CS_LAUNCH(k_r3_quot_l2<Rep3Pol<FrP>>, ceil_div(n4, 64), 64, 0, st, qi, s->B, E, n, pk->nlag, s->K, s->party, s->prf, s->ctr,
                 s->arena.as<uint32_t>(), s->slot_words, t, tz);
       s->ctr += 2 * (uint64_t)n4;
       CS_TRY(ntt_run(ctx, pk->dom4, t, 1, true, nullptr, st));
@@ -762,42 +780,12 @@ int r3_step_t(cs_plonk_rep3* s, int step, const uint64_t* h_in, uint64_t* h_out)
     case CS_PLONK_R3_ROUND5: {  // in: xi, v0, eval_a eval_b eval_c eval_s1 eval_s2 eval_zw (opened); out: partial [Wxi] [Wxiw]
       HR in[8];
       memcpy(in, h_in, sizeof(in));
-      const HR xi = in[0], ea = in[2], eb = in[3], ec = in[4], es1 = in[5], es2 = in[6], ezw = in[7];
-      HR v[5], beta, gamma, alpha, alpha2, k1, k2, w_n;
-      v[0] = in[1];
-      for (int i = 1; i < 5; i++) v[i] = v[i - 1] * v[0];
-      memcpy(beta.l, s->K.beta, 32); memcpy(gamma.l, s->K.gamma, 32); memcpy(alpha.l, s->K.alpha, 32); memcpy(alpha2.l, s->K.alpha2, 32);
-      memcpy(k1.l, s->K.k1, 32); memcpy(k2.l, s->K.k2, 32);
+      const HR xi = in[0], ezw = in[7];
+      HR w_n;
       memcpy(w_n.l, pk->dom->group_gen.data(), sizeof(w_n.l));
       const HR xiw = xi * w_n;
-      HR xin = xi;
-      for (unsigned q = 0; q < pk->log_n; q++) xin = xin.sqr();
-      const HR zh = xin - HR::one(), nn = HR::from_u64(n);
-      std::vector<HR> ls(pk->nlag);
-      HR wi = HR::one();
-      for (uint32_t i = 0; i < pk->nlag; i++) {
-        HR dnm = nn * (xi - wi);
-        if (dnm.is_zero()) return fail(CS_ERR_ARG, "plonk: xi hit the evaluation domain");
-        ls[i] = wi * zh * dnm.inverse();
-        wi = wi * w_n;
-      }
-      HR eval_pi = HR::zero();
-      for (uint32_t i = 0; i < pk->n_public && i < pk->nlag; i++) {
-        HR val;
-        memcpy(val.l, s->pub.data() + (size_t)i * HR::N, sizeof(val.l));
-        eval_pi = eval_pi - ls[i] * val;
-      }
-      const HR betaxi = beta * xi;
-      const HR e2 = (ea + betaxi + gamma) * (eb + betaxi * k1 + gamma) * (ec + betaxi * k2 + gamma) * alpha;
-      const HR e3 = (ea + beta * es1 + gamma) * (eb + beta * es2 + gamma) * ezw * alpha;
-      const HR e4 = alpha2 * ls[0];
-      const HR r0 = eval_pi - e3 * (ec + gamma) - e4;
       PlonkLinW W;
-      memset(&W, 0, sizeof(W));
-      put(W.ab, ea * eb); put(W.ea, ea); put(W.eb, eb); put(W.ec, ec); put(W.e3beta, e3 * beta); put(W.e24, e2 + e4);
-      put(W.zh, zh); put(W.xin, xin); put(W.xin2, xin.sqr());
-      for (int i = 0; i < 5; i++) put(W.v[i], v[i]);
-      put(W.c0, r0 - v[0] * ea - v[1] * eb - v[2] * ec - v[3] * es1 - v[4] * es2);
+      CS_TRY(lin_weights<Cfg>(pk, s->pub.data(), s->K, xi, in[1], in + 2, W));
       PlonkLinIn li;
       li.qm = pk->q_coeffs[0].as<uint32_t>(); li.ql = pk->q_coeffs[1].as<uint32_t>(); li.qr = pk->q_coeffs[2].as<uint32_t>();
       li.qo = pk->q_coeffs[3].as<uint32_t>(); li.qc = pk->q_coeffs[4].as<uint32_t>();
@@ -1011,6 +999,272 @@ int r3_prove_t(cs_plonk_rep3* s, cs_net* net, cs_rep3_state* state, const uint64
 
 }  // namespace
 
+// ======================================================================================================
+// Shamir co-Plonk (ShamirCoPlonk::prove, co-plonk/src/lib.rs:237-260 with ShamirPlonkDriver, mpc/shamir.rs): one
+// session per party of a Shamir(n, t) sharing, the whole proof inside the library over a cs_net.  A share is one Fr
+// element, so every linear step -- additions, gather, iNTT / extension, blinding, tsplit, evaluation, the Wxi numerator,
+// division by (X - xi), the commitments -- is the plain prover's kernel on shares, with public values added by every
+// party.  Products follow the Rep3 session's layering (cs_plonk_rep3.cuh, ShamirPol): a local product (degree 2t), then
+// ONE device degree reduction per product layer covering all of its slots (one king round each):
+//   round 2  n12 d12 | num den | x u | m      7n reductions; G = den s, Q = r s' and Y = m / r_{i+1} open at degree 2t;
+//            s, r, s' are 3n + 2 random shares (the r_t halves of double sharings)
+//   round 3  the twelve first-layer products  48n reductions; t and tz stay at degree 2t
+// Degree-2t results (T1 T2 T3 Wxi) open with 2t + 1 parties; a b c Z Wxiw and the four evaluations with t + 1.
+// Pairs per proof: 10n + 2 (made on the device when round 2 starts) + 48n (when round 3 starts) = 58n + 2, plus the
+// 11 blinders from the state's host pool (ShamirState::rand) unless the caller brings them: 58n + 13.
+// ======================================================================================================
+struct cs_plonk_shamir {
+  cs_ctx* ctx = nullptr;
+  cs_plonk_pk* pk = nullptr;
+  int n_parties = 0, thr = 0, party = 0;
+  cs_shamir_state* state = nullptr;  // created over the first proof's net, kept for the next ones
+  DevBuf w, buf[3], poly[4], ev[4], arena, pair_t, pair_2t, addv, pubv, t, tz, t1, t2, t3, tmp0, tmp1, totals, small;
+  size_t pairs = 0;    // pairs the last proof consumed
+  double pair_ms = 0;  // wall time of the last proof's device pair generation
+};
+
+namespace {
+
+template <class Cfg>
+int sh_create_t(cs_plonk_shamir* s) {
+  const cs_plonk_pk* pk = s->pk;
+  const size_t n = pk->n;
+  CS_TRY(s->w.reserve((size_t)pk->n_vars * 32));
+  for (int i = 0; i < 3; i++) CS_TRY(s->buf[i].reserve(n * 32));
+  for (int i = 0; i < 4; i++) {
+    CS_TRY(s->poly[i].reserve((n + 8) * 32));
+    CS_TRY(s->ev[i].reserve(4 * n * 32));
+  }
+  CS_TRY(s->arena.reserve(48 * n * 32));  // round 3: twelve slots of 4n; round 2: seven slots of n
+  CS_TRY(s->addv.reserve((2 * n + 2) * 32));
+  CS_TRY(s->pubv.reserve((8 * n + 16) * 32));  // 1/G | 1/Q | scan scratch | opened G | Q
+  CS_TRY(s->t.reserve(4 * n * 32));
+  CS_TRY(s->tz.reserve(4 * n * 32));
+  CS_TRY(s->t1.reserve((n + 8) * 32));
+  CS_TRY(s->t2.reserve((n + 8) * 32));
+  CS_TRY(s->t3.reserve((n + 8) * 32));
+  CS_TRY(s->tmp0.reserve((n + 8) * 32));
+  CS_TRY(s->tmp1.reserve((n + 8) * 32));
+  CS_TRY(s->small.reserve(8192));
+  return 0;
+}
+
+template <class Cfg>
+int sh_prove_t(cs_plonk_shamir* s, cs_net* net, const uint64_t* h_pub, const uint64_t* h_wit, const uint64_t* h_blind,
+               uint64_t* out_points, uint64_t* out_evals, uint64_t* out_blind) {
+  typedef typename Cfg::FrP FrP;
+  typedef host::HFp<FrP> HR;
+  typedef ShamirPol<FrP> Pol;
+  constexpr int NW = FrP::N;
+  cs_ctx* ctx = s->ctx;
+  cs_plonk_pk* pk = s->pk;
+  cudaStream_t st = ctx->stream;
+  const cs_curve cv = (cs_curve)pk->curve;
+  const uint32_t n = pk->n, n4 = 4 * n, npub = pk->n_public;
+  const size_t pl = point_limbs64(pk->curve, CS_G1);
+  const unsigned gb = ceil_div(n, 128);
+  s->pairs = 0;
+  s->pair_ms = 0;
+  if (!s->state) CS_TRY(cs_shamir_state_create(net, cv, s->n_parties, s->thr, 0, &s->state));
+  cs_shamir_state* sst = s->state;
+  // Round1Challenges::random (round1.rs:82-92): eleven ShamirState::rand shares unless the caller brings them
+  HR b[11];
+  if (h_blind) memcpy(b, h_blind, sizeof(b));
+  else {
+    for (int i = 0; i < 11; i++) CS_TRY(cs_shamir_state_rand(sst, net, b[i].l));
+    s->pairs += 11;
+  }
+  if (out_blind) memcpy(out_blind, b, sizeof(b));
+  auto make_pairs = [&](size_t count) -> int {
+    CS_TRY(s->pair_t.reserve(count * 32));
+    CS_TRY(s->pair_2t.reserve(count * 32));
+    const auto t0 = std::chrono::steady_clock::now();
+    CS_TRY(shamir_double_sharings(ctx, sst, net, count, s->pair_t.as<uint64_t>(), s->pair_2t.as<uint64_t>()));
+    s->pair_ms += std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
+    s->pairs += count;
+    return 0;
+  };
+  auto reduce = [&](uint32_t* v, size_t len, size_t first_pair) {  // in place, pairs [first_pair, first_pair + len)
+    CS_CUDA(cudaStreamSynchronize(st));
+    return shamir_degree_reduce(ctx, sst, net, (const uint64_t*)v, len, (uint64_t*)v, s->pair_t.as<uint64_t>() + first_pair * 4,
+                                s->pair_2t.as<uint64_t>() + first_pair * 4);
+  };
+  auto open_points = [&](uint64_t* p, int k, int degree_2t) {
+    return shamir_open_points(sst, net, CS_G1, degree_2t, p, k);
+  };
+  // ---- init round (round1.rs:191-252): w = 0 | public (every party holds the value itself) | witness shares | additions
+  uint32_t* w = s->w.as<uint32_t>();
+  const uint32_t n_priv = pk->n_vars - pk->n_additions - npub - 1;
+  CS_CUDA(cudaMemsetAsync(w, 0, 32, st));
+  if (npub) CS_CUDA(cudaMemcpyAsync(w + NW, h_pub + HR::N, (size_t)npub * 32, cudaMemcpyHostToDevice, st));
+  if (n_priv) CS_CUDA(cudaMemcpyAsync(w + (size_t)(npub + 1) * NW, h_wit, (size_t)n_priv * 32, cudaMemcpyHostToDevice, st));
+  {
+    uint32_t lo = 0;
+    for (uint32_t hi : pk->level_ends) {
+      CS_LAUNCH(k_plonk_additions<FrP>, ceil_div(hi - lo, 128), 128, 0, st, pk->add_order.as<uint32_t>(), lo, hi,
+                pk->add_ids.as<uint32_t>(), pk->add_factors.as<uint32_t>(), pk->n_vars - pk->n_additions, 1u, w);
+      lo = hi;
+    }
+  }
+  // ---- round 1
+  const uint32_t* maps[3] = {pk->map_a.as<uint32_t>(), pk->map_b.as<uint32_t>(), pk->map_c.as<uint32_t>()};
+  uint32_t *buf[3], *poly[4], *ev[4];
+  for (int i = 0; i < 3; i++) buf[i] = s->buf[i].as<uint32_t>();
+  for (int i = 0; i < 4; i++) { poly[i] = s->poly[i].as<uint32_t>(); ev[i] = s->ev[i].as<uint32_t>(); }
+  for (int k = 0; k < 3; k++) {
+    CS_LAUNCH(k_plonk_gather<FrP>, ceil_div(n, 256), 256, 0, st, maps[k], pk->n_constraints, n, 1u, w, buf[k]);
+    CS_CUDA(cudaMemcpyAsync(poly[k], buf[k], (size_t)n * 32, cudaMemcpyDeviceToDevice, st));
+    CS_TRY(interpolate_and_extend<Cfg>(ctx, pk, poly[k], ev[k]));
+    CS_TRY(blind<Cfg>(ctx, poly[k], n, b + 2 * k, 2));
+  }
+  uint64_t* P = out_points;  // A B C Z T1 T2 T3 Wxi Wxiw
+  {
+    Commit c[3] = {{poly[0], (size_t)n + 2, P}, {poly[1], (size_t)n + 2, P + pl}, {poly[2], (size_t)n + 2, P + 2 * pl}};
+    CS_TRY(commit_many<Cfg>(ctx, pk, c, 3));
+  }
+  CS_TRY(open_points(P, 3, 0));
+  // ---- round 2 (round2.rs:197-250)
+  HR k1, k2;
+  memcpy(k1.l, pk->k1.data(), sizeof(k1.l));
+  memcpy(k2.l, pk->k2.data(), sizeof(k2.l));
+  Transcript<Cfg> tr;
+  for (int i = 0; i < 8; i++) tr.add_point(pk->vk_points.data() + i * pl);
+  for (uint32_t i = 0; i < npub; i++) {
+    HR v;
+    memcpy(v.l, h_pub + (size_t)(i + 1) * HR::N, sizeof(v.l));
+    tr.add_scalar(v);
+  }
+  for (int i = 0; i < 3; i++) tr.add_point(P + i * pl);
+  const HR beta = tr.get_challenge();
+  tr = Transcript<Cfg>();
+  tr.add_scalar(beta);
+  const HR gamma = tr.get_challenge();
+  PlonkConsts K;
+  memset(&K, 0, sizeof(K));
+  for (int i = 0; i < 11; i++) put(K.b[i], b[i]);
+  put(K.beta, beta); put(K.gamma, gamma); put(K.k1, k1); put(K.k2, k2);
+  const uint32_t* tw4 = pk->dom4->tw_fwd.template as<uint32_t>();
+  CS_TRY(make_pairs(10 * (size_t)n + 2));
+  const ShamirRnd R{s->pair_t.as<uint32_t>()};  // s, r, s' = the r_t halves of pairs [0, 3n + 2)
+  const size_t first = 3 * (size_t)n + 2;         // the reductions take the pairs after them
+  uint32_t* arena = s->arena.as<uint32_t>();
+  auto slot = [&](int k) { return arena + (size_t)k * n * NW; };  // round 2: slots of n, a layer's slots adjacent
+  uint32_t *pubv = s->pubv.as<uint32_t>(), *addv = s->addv.as<uint32_t>();
+  uint32_t *ginv = pubv, *qinv = pubv + (size_t)n * NW, *pscr = pubv + (size_t)(2 * n + 1) * NW;
+  uint32_t* opened = pscr + (size_t)(4 * n + 4) * NW;
+  R3Round2In in;
+  in.a = buf[0]; in.b = buf[1]; in.c = buf[2];
+  in.s1 = pk->s_evals[0].as<uint32_t>(); in.s2 = pk->s_evals[1].as<uint32_t>(); in.s3 = pk->s_evals[2].as<uint32_t>();
+  in.tw4 = tw4;
+  uint32_t* none = nullptr;
+  CS_LAUNCH(k_r3_round2_a<Pol>, gb, 128, 0, st, in, K, n, s->party, R, 0ull, slot(0), slot(1), none, none);
+  CS_TRY(reduce(slot(0), 2 * (size_t)n, first));
+  CS_LAUNCH(k_r3_round2_b<Pol>, gb, 128, 0, st, in, K, n, s->party, R, 0ull, slot(0), slot(1), slot(2), slot(3), none, none);
+  CS_TRY(reduce(slot(2), 2 * (size_t)n, first + 2 * (size_t)n));
+  CS_LAUNCH(k_r3_round2_c<Pol>, ceil_div(n + 1, 128), 128, 0, st, slot(3), n, R, 0ull, 0ull, addv, addv + (size_t)n * NW);
+  CS_CUDA(cudaStreamSynchronize(st));
+  CS_TRY(shamir_open_vec(ctx, sst, net, 1, (const uint64_t*)addv, 2 * (size_t)n + 1, (uint64_t*)opened));
+  CS_TRY(r3_batch_inverse<Cfg>(s, opened, n, pscr, ginv));
+  CS_TRY(r3_batch_inverse<Cfg>(s, opened + (size_t)n * NW, n + 1, pscr, qinv));
+  CS_LAUNCH(k_r3_round2_d<Pol>, gb, 128, 0, st, slot(2), ginv, qinv, n, R, 0ull, 0ull, slot(4), slot(5), none, none);
+  CS_TRY(reduce(slot(4), 2 * (size_t)n, first + 4 * (size_t)n));
+  CS_LAUNCH(k_r3_round2_e<Pol>, gb, 128, 0, st, slot(4), n, R, 0ull, 0ull, slot(6), none);
+  CS_TRY(reduce(slot(6), n, first + 6 * (size_t)n));
+  CS_LAUNCH(k_r3_round2_f<Pol>, gb, 128, 0, st, slot(6), qinv, n, R, 0ull, 0ull, addv);
+  CS_CUDA(cudaStreamSynchronize(st));
+  uint32_t* y = pscr;
+  CS_TRY(shamir_open_vec(ctx, sst, net, 1, (const uint64_t*)addv, n, (uint64_t*)y));
+  CS_TRY((scan<FrP, 0>(ctx, s, y, y, n, 0)));
+  CS_LAUNCH(k_r3_round2_g<Pol>, gb, 128, 0, st, y, slot(5), n, poly[3]);
+  CS_TRY(interpolate_and_extend<Cfg>(ctx, pk, poly[3], ev[3]));
+  CS_TRY(blind<Cfg>(ctx, poly[3], n, b + 6, 3));
+  {
+    Commit c[1] = {{poly[3], (size_t)n + 3, P + 3 * pl}};
+    CS_TRY(commit_many<Cfg>(ctx, pk, c, 1));
+  }
+  CS_TRY(open_points(P + 3 * pl, 1, 0));
+  // ---- round 3 (round3.rs:560-610)
+  tr = Transcript<Cfg>();
+  tr.add_scalar(beta);
+  tr.add_scalar(gamma);
+  tr.add_point(P + 3 * pl);
+  const HR alpha = tr.get_challenge();
+  const HR alpha2 = alpha.sqr();
+  put(K.alpha, alpha); put(K.alpha2, alpha2);
+  CS_TRY(quotient_consts<Cfg>(pk->curve, K));
+  CS_TRY(make_pairs(48 * (size_t)n));
+  R3QuotIn qi;
+  qi.a = ev[0]; qi.b = ev[1]; qi.c = ev[2]; qi.z = ev[3]; qi.tw4 = tw4;
+  R3Blinders B;
+  memset(&B, 0, sizeof(B));
+  for (int i = 0; i < 9; i++) put(B.b[i].v[0], b[i]);
+  const size_t slot_words = (size_t)n4 * NW;
+  const ShamirRnd R3{nullptr};  // round 3 draws no random shares; round 2's pair buffer has been replaced
+  CS_LAUNCH(k_r3_quot_l1<Pol>, ceil_div(n4, 64), 64, 0, st, qi, B, n, R3, 0ull, arena, none, slot_words);
+  CS_TRY(reduce(arena, 12 * (size_t)n4, 0));
+  R3KeyEvals E;
+  E.qm = pk->q_evals[0].as<uint32_t>(); E.ql = pk->q_evals[1].as<uint32_t>(); E.qr = pk->q_evals[2].as<uint32_t>();
+  E.qo = pk->q_evals[3].as<uint32_t>(); E.qc = pk->q_evals[4].as<uint32_t>();
+  E.s1 = pk->s_evals[0].as<uint32_t>(); E.s2 = pk->s_evals[1].as<uint32_t>(); E.s3 = pk->s_evals[2].as<uint32_t>();
+  E.lagrange = pk->lagrange.as<uint32_t>(); E.buf_a = buf[0];
+  uint32_t *t = s->t.as<uint32_t>(), *tz = s->tz.as<uint32_t>();
+  CS_LAUNCH(k_r3_quot_l2<Pol>, ceil_div(n4, 64), 64, 0, st, qi, B, E, n, pk->nlag, K, s->party, R3, 0ull, arena, slot_words, t, tz);
+  CS_TRY(ntt_run(ctx, pk->dom4, t, 1, true, nullptr, st));
+  CS_TRY(ntt_run(ctx, pk->dom4, tz, 1, true, nullptr, st));
+  CS_LAUNCH(k_bit_reverse<FrP>, ceil_div(n4, 256), 256, 0, st, t, pk->log_n + 2, 1u);
+  CS_LAUNCH(k_bit_reverse<FrP>, ceil_div(n4, 256), 256, 0, st, tz, pk->log_n + 2, 1u);
+  uint32_t *t1 = s->t1.as<uint32_t>(), *t2 = s->t2.as<uint32_t>(), *t3 = s->t3.as<uint32_t>();
+  CS_LAUNCH(k_plonk_tsplit<FrP>, gb, 128, 0, st, t, tz, n, K, t1, t2, t3);
+  {
+    Commit c[3] = {{t1, (size_t)n + 1, P + 4 * pl}, {t2, (size_t)n + 1, P + 5 * pl}, {t3, (size_t)n + 6, P + 6 * pl}};
+    CS_TRY(commit_many<Cfg>(ctx, pk, c, 3));
+  }
+  CS_TRY(open_points(P + 4 * pl, 3, 1));
+  // ---- round 4 (round4.rs:108-165)
+  tr = Transcript<Cfg>();
+  tr.add_scalar(alpha);
+  for (int i = 4; i < 7; i++) tr.add_point(P + i * pl);
+  const HR xi = tr.get_challenge();
+  HR w_n;
+  memcpy(w_n.l, pk->dom->group_gen.data(), sizeof(w_n.l));
+  const HR xiw = xi * w_n;
+  HR ev4[4], es1, es2;  // a b c zw (shares, then opened)
+  for (int k = 0; k < 3; k++) CS_TRY((eval_poly_t<Cfg>(ctx, reinterpret_cast<uint64_t*>(poly[k]), (size_t)n + 2, 1, xi.l, ev4[k].l)));
+  CS_TRY((eval_poly_t<Cfg>(ctx, reinterpret_cast<uint64_t*>(poly[3]), (size_t)n + 3, 1, xiw.l, ev4[3].l)));
+  CS_TRY((eval_poly_t<Cfg>(ctx, pk->s_coeffs[0].as<uint64_t>(), (size_t)n, 1, xi.l, es1.l)));
+  CS_TRY((eval_poly_t<Cfg>(ctx, pk->s_coeffs[1].as<uint64_t>(), (size_t)n, 1, xi.l, es2.l)));
+  CS_TRY(shamir_open_scalars(sst, net, 0, ev4[0].l, 4));
+  const HR ea = ev4[0], eb = ev4[1], ec = ev4[2], ezw = ev4[3];
+  // ---- round 5 (round5.rs:284-340)
+  tr = Transcript<Cfg>();
+  tr.add_scalar(xi); tr.add_scalar(ea); tr.add_scalar(eb); tr.add_scalar(ec);
+  tr.add_scalar(es1); tr.add_scalar(es2); tr.add_scalar(ezw);
+  const HR evs5[6] = {ea, eb, ec, es1, es2, ezw};
+  PlonkLinW W;
+  CS_TRY(lin_weights<Cfg>(pk, h_pub + HR::N, K, xi, tr.get_challenge(), evs5, W));
+  PlonkLinIn li;
+  li.qm = pk->q_coeffs[0].as<uint32_t>(); li.ql = pk->q_coeffs[1].as<uint32_t>(); li.qr = pk->q_coeffs[2].as<uint32_t>();
+  li.qo = pk->q_coeffs[3].as<uint32_t>(); li.qc = pk->q_coeffs[4].as<uint32_t>();
+  li.s1 = pk->s_coeffs[0].as<uint32_t>(); li.s2 = pk->s_coeffs[1].as<uint32_t>(); li.s3 = pk->s_coeffs[2].as<uint32_t>();
+  li.pa = poly[0]; li.pb = poly[1]; li.pc = poly[2]; li.pz = poly[3]; li.t1 = t1; li.t2 = t2; li.t3 = t3;
+  uint32_t *wxi = s->tmp0.as<uint32_t>(), *wxiw = s->tmp1.as<uint32_t>();
+  CS_LAUNCH(k_plonk_wxi_numerator<FrP>, ceil_div(n + 6, 128), 128, 0, st, li, W, n, 1, wxi);  // pub = 1 at every party
+  CS_TRY(divide_by_linear<Cfg>(ctx, s, wxi, n + 6, xi, (const HR*)nullptr));
+  CS_CUDA(cudaMemcpyAsync(wxiw, poly[3], (size_t)(n + 3) * 32, cudaMemcpyDeviceToDevice, st));
+  CS_TRY(divide_by_linear<Cfg>(ctx, s, wxiw, n + 3, xiw, &ezw));
+  {
+    Commit c[2] = {{wxi, (size_t)n + 5, P + 7 * pl}, {wxiw, (size_t)n + 2, P + 8 * pl}};
+    CS_TRY(commit_many<Cfg>(ctx, pk, c, 2));
+  }
+  CS_TRY(open_points(P + 7 * pl, 1, 1));  // Wxi: degree 2t (it carries T1 T2 T3)
+  CS_TRY(open_points(P + 8 * pl, 1, 0));  // Wxiw: degree t
+  const HR evs[6] = {ea, eb, ec, es1, es2, ezw};
+  memcpy(out_evals, evs, sizeof(evs));
+  return 0;
+}
+
+}  // namespace
+
 extern "C" {
 
 int cs_plonk_pk_create(cs_ctx* ctx, const cs_plonk_key_desc* d, cs_plonk_pk** out) {
@@ -1213,6 +1467,74 @@ int cs_plonk_rep3_prove(cs_plonk_rep3* s, cs_net* net, cs_rep3_state* state, con
 #endif
     default: return fail(CS_ERR_ARG, "unsupported curve id %d", s->pk->curve);
   }
+}
+
+int cs_plonk_shamir_create(cs_ctx* ctx, cs_plonk_pk* pk, int num_parties, int threshold, int party, cs_plonk_shamir** out) {
+  if (!ctx || !pk || !out) return fail(CS_ERR_ARG, "cs_plonk_shamir_create: NULL argument");
+  if (threshold < 1 || 2 * threshold + 1 > num_parties) return fail(CS_ERR_ARG, "Threshold too large for number of parties");
+  if (num_parties > (int)LINCOMB_MAX) return fail(CS_ERR_LIMIT, "cs_plonk_shamir_create: %d parties exceed %u", num_parties, LINCOMB_MAX);
+  if (party < 0 || party >= num_parties) return fail(CS_ERR_ARG, "cs_plonk_shamir_create: party id %d of %d", party, num_parties);
+  CS_CUDA(cudaSetDevice(ctx->device));
+  std::unique_ptr<cs_plonk_shamir> s(new cs_plonk_shamir());
+  s->ctx = ctx; s->pk = pk; s->n_parties = num_parties; s->thr = threshold; s->party = party;
+  int rc = pk->curve == CS_BN254 ? sh_create_t<Bn254Cfg>(s.get())
+#if defined(CS_ENABLE_BLS12_381)
+           : pk->curve == CS_BLS12_381 ? sh_create_t<Bls381Cfg>(s.get())
+#endif
+           : fail(CS_ERR_ARG, "unsupported curve id %d", pk->curve);
+  if (rc) { cs_plonk_shamir_free(s.release()); return rc; }
+  *out = s.release();
+  return 0;
+}
+
+void cs_plonk_shamir_free(cs_plonk_shamir* s) {
+  if (!s) return;
+  DevBuf* all[] = {&s->w, &s->arena, &s->pair_t, &s->pair_2t, &s->addv, &s->pubv, &s->t, &s->tz, &s->t1, &s->t2, &s->t3,
+                   &s->tmp0, &s->tmp1, &s->totals, &s->small};
+  for (DevBuf* b : all) b->release();
+  for (int i = 0; i < 3; i++) s->buf[i].release();
+  for (int i = 0; i < 4; i++) { s->poly[i].release(); s->ev[i].release(); }
+  cs_shamir_state_free(s->state);
+  delete s;
+}
+
+int cs_plonk_shamir_prove(cs_plonk_shamir* s, cs_net* net, const uint64_t* h_public_inputs, size_t n_public_inputs,
+                          const uint64_t* h_witness_shares, size_t n_witness, const uint64_t* h_blinder_shares,
+                          uint64_t* out_points, uint64_t* out_evals, uint64_t* out_blinder_shares) {
+  if (!s || !net || !h_public_inputs || !out_points || !out_evals || (n_witness && !h_witness_shares))
+    return fail(CS_ERR_ARG, "cs_plonk_shamir_prove: NULL argument");
+  if (net->n != s->n_parties || net->id != s->party)
+    return fail(CS_ERR_ARG, "cs_plonk_shamir_prove: the net is party %d of %d, the session is party %d of %d", net->id, net->n,
+                s->party, s->n_parties);
+  const cs_plonk_pk* pk = s->pk;
+  if (n_public_inputs != (size_t)pk->n_public + 1)
+    return fail(CS_ERR_ARG, "cs_plonk_shamir_prove: %zu public inputs, the key expects %u", n_public_inputs, pk->n_public + 1);
+  if (n_witness != (size_t)pk->n_vars - pk->n_additions - pk->n_public - 1)
+    return fail(CS_ERR_ARG, "cs_plonk_shamir_prove: %zu witness shares, the key expects %u", n_witness,
+                pk->n_vars - pk->n_additions - pk->n_public - 1);
+  CS_CUDA(cudaSetDevice(s->ctx->device));
+  switch (pk->curve) {
+    case CS_BN254: return sh_prove_t<Bn254Cfg>(s, net, h_public_inputs, h_witness_shares, h_blinder_shares, out_points, out_evals, out_blinder_shares);
+#if defined(CS_ENABLE_BLS12_381)
+    case CS_BLS12_381: return sh_prove_t<Bls381Cfg>(s, net, h_public_inputs, h_witness_shares, h_blinder_shares, out_points, out_evals, out_blinder_shares);
+#endif
+    default: return fail(CS_ERR_ARG, "unsupported curve id %d", pk->curve);
+  }
+}
+
+size_t cs_plonk_shamir_pairs(const cs_plonk_shamir* s) { return s ? s->pairs : 0; }
+
+double cs_plonk_shamir_pair_ms(const cs_plonk_shamir* s) { return s ? s->pair_ms : 0.0; }
+
+size_t cs_plonk_shamir_device_bytes(const cs_plonk_shamir* s) {
+  if (!s) return 0;
+  const DevBuf* all[] = {&s->w, &s->arena, &s->pair_t, &s->pair_2t, &s->addv, &s->pubv, &s->t, &s->tz, &s->t1, &s->t2, &s->t3,
+                         &s->tmp0, &s->tmp1, &s->totals, &s->small};
+  size_t b = shamir_state_device_bytes(s->state);
+  for (const DevBuf* x : all) b += x->cap;
+  for (int i = 0; i < 3; i++) b += s->buf[i].cap;
+  for (int i = 0; i < 4; i++) b += s->poly[i].cap + s->ev[i].cap;
+  return b;
 }
 
 }  // extern "C"

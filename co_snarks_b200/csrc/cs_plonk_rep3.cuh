@@ -13,6 +13,10 @@
 //            evaluations everything is linear, so rounds 3b-5 run the plain kernels on additive shares.
 // The opened proof equals the plain prover's for blinders b = sum of the parties' shares (masks cancel), which
 // is what the parity tests check.
+//
+// The Shamir session (cs_plonk_shamir) runs the same kernel bodies over ShamirPol: a share is one element of a
+// degree-t sharing, a product is the plain local product (degree 2t) and the caller degree-reduces each product layer
+// with one king round; the layer above the last reduction (t, tz in round 3) stays at degree 2t.
 #pragma once
 #include "cs_plonk.cuh"
 #include "cs_prf.cuh"
@@ -72,97 +76,152 @@ template <class FrP> CS_D Sh<FrP> prf_share(const PrfArgs& P, uint64_t rbase, ui
   return Sh<FrP>{prf_field_element_wide<FrP>(P.keys.k, P.pos1 + w, P.rounds), prf_field_element_wide<FrP>(P.keys.k + 8, P.pos2 + w, P.rounds)};
 }
 
+// ---- share policies -------------------------------------------------------------------------------------
+// The round-2/3 kernels below are written once over a share policy:
+//   Rep3Pol<FrP>    replicated {a, b}; a product is the masked cross-term sum, stored into this party's .a and the
+//                   next party's .b; random shares come from the correlated ChaCha streams; public values enter the
+//                   x_0 component; the additive part of a linear expression is .a
+//   ShamirPol<FrP>  one Fr element of a degree-t sharing; a product is the plain local product (degree 2t, reduced by
+//                   the caller); random shares are r_t halves of device double sharings; every party adds public values
+template <class FrP_>
+struct Rep3Pol {
+  typedef FrP_ FrP;
+  typedef Fp<FrP> F;
+  typedef Sh<FrP> S;
+  typedef PrfArgs Rnd;
+  static CS_D S ld(const uint32_t* p, size_t i) { return ld_sh<FrP>(p, i); }
+  static CS_D void st(uint32_t* p, size_t i, const S& s) { st_sh<FrP>(p, i, s); }
+  static CS_D S cnst(const ShConst& c) { return sh_const<FrP>(c); }
+  static CS_D S add(const S& x, const S& y) { return sh_add<FrP>(x, y); }
+  static CS_D S mulp(const S& x, const F& p) { return sh_mulp<FrP>(x, p); }
+  static CS_D S addp(const S& x, const F& p, int party) { return sh_addp<FrP>(x, p, party); }
+  static CS_D F lmul(const S& x, const S& y) { return sh_lmul<FrP>(x, y); }
+  static CS_D F part(const S& x) { return x.a; }
+  static CS_D bool pub(int party) { return party == 0; }
+  static CS_D F masked(const F& z, const Rnd& P, uint64_t idx) { return z + prf_mask<FrP>(P, idx); }
+  static CS_D S rand(const Rnd& P, uint64_t rbase, uint64_t j) { return prf_share<FrP>(P, rbase, j); }
+  static CS_D void st_prod(uint32_t* mine, uint32_t* next, size_t i, const F& z) { st_reshare<FrP>(mine, next, i, z); }
+};
+struct ShamirRnd { const uint32_t* r; };  // random degree-t shares
+template <class FrP_>
+struct ShamirPol {
+  typedef FrP_ FrP;
+  typedef Fp<FrP> F;
+  typedef Fp<FrP> S;
+  typedef ShamirRnd Rnd;
+  static CS_D S ld(const uint32_t* p, size_t i) { return ld_fr<FrP>(p + i * FrP::N); }
+  static CS_D void st(uint32_t* p, size_t i, const S& s) { st_fr<FrP>(p + i * FrP::N, s); }
+  static CS_D S cnst(const ShConst& c) { return cload<FrP>(c.v[0]); }
+  static CS_D S add(const S& x, const S& y) { return x + y; }
+  static CS_D S mulp(const S& x, const F& p) { return x * p; }
+  static CS_D S addp(const S& x, const F& p, int) { return x + p; }
+  static CS_D F lmul(const S& x, const S& y) { return x * y; }
+  static CS_D F part(const S& x) { return x; }
+  static CS_D bool pub(int) { return true; }
+  static CS_D F masked(const F& z, const Rnd&, uint64_t) { return z; }
+  static CS_D S rand(const Rnd& P, uint64_t rbase, uint64_t j) { return ld_fr<FrP>(P.r + (rbase + j) * FrP::N); }
+  static CS_D void st_prod(uint32_t* mine, uint32_t*, size_t i, const F& z) { st_fr<FrP>(mine + i * FrP::N, z); }
+};
+
 struct R3Round2In {
   const uint32_t *a, *b, *c;        // wire buffers, n shares each
   const uint32_t *s1, *s2, *s3;     // sigma evaluations (4n, read at stride 4)
   const uint32_t* tw4;
 };
 // numerator / denominator factors of z (round2.rs:113-146), k = 0..2
-template <class FrP>
-CS_D void r3_factors(const R3Round2In& in, const PlonkConsts& K, uint32_t n, uint32_t i, int party, int k, Sh<FrP>& nf, Sh<FrP>& df) {
+template <class Pol>
+CS_D void r3_factors(const R3Round2In& in, const PlonkConsts& K, uint32_t n, uint32_t i, int party, int k, typename Pol::S& nf,
+                     typename Pol::S& df) {
+  typedef typename Pol::FrP FrP;
   typedef Fp<FrP> F;
   constexpr int NW = FrP::N;
   F beta = cload<FrP>(K.beta), gamma = cload<FrP>(K.gamma);
   F bw = beta * root_pow<FrP>(in.tw4, 2 * n, 4 * i);
   const uint32_t* wire = k == 0 ? in.a : (k == 1 ? in.b : in.c);
   const uint32_t* sig = k == 0 ? in.s1 : (k == 1 ? in.s2 : in.s3);
-  Sh<FrP> x = ld_sh<FrP>(wire, i);
+  typename Pol::S x = Pol::ld(wire, i);
   F kk = k == 0 ? F::one() : cload<FrP>(k == 1 ? K.k1 : K.k2);
-  nf = sh_addp<FrP>(x, kk * bw + gamma, party);
-  df = sh_addp<FrP>(x, beta * ld_fr<FrP>(sig + (size_t)(4 * i) * NW) + gamma, party);
+  nf = Pol::addp(x, kk * bw + gamma, party);
+  df = Pol::addp(x, beta * ld_fr<FrP>(sig + (size_t)(4 * i) * NW) + gamma, party);
 }
 
 // layer 1: n12 = n1 n2, d12 = d1 d2  -> slots o_n, o_d (reshared)
-template <class FrP>
-CS_GLOBAL void k_r3_round2_a(R3Round2In in, PlonkConsts K, uint32_t n, int party, PrfArgs P, uint64_t mbase,
+template <class Pol>
+CS_GLOBAL void k_r3_round2_a(R3Round2In in, PlonkConsts K, uint32_t n, int party, typename Pol::Rnd P, uint64_t mbase,
                               uint32_t* on, uint32_t* od, uint32_t* pn, uint32_t* pd) {
   uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
-  Sh<FrP> n1, d1, n2, d2;
-  r3_factors<FrP>(in, K, n, i, party, 0, n1, d1);
-  r3_factors<FrP>(in, K, n, i, party, 1, n2, d2);
-  st_reshare<FrP>(on, pn, i, sh_lmul<FrP>(n1, n2) + prf_mask<FrP>(P, mbase + i));
-  st_reshare<FrP>(od, pd, i, sh_lmul<FrP>(d1, d2) + prf_mask<FrP>(P, mbase + n + i));
+  typename Pol::S n1, d1, n2, d2;
+  r3_factors<Pol>(in, K, n, i, party, 0, n1, d1);
+  r3_factors<Pol>(in, K, n, i, party, 1, n2, d2);
+  Pol::st_prod(on, pn, i, Pol::masked(Pol::lmul(n1, n2), P, mbase + i));
+  Pol::st_prod(od, pd, i, Pol::masked(Pol::lmul(d1, d2), P, mbase + n + i));
 }
 // layer 2: num = n12 n3, den = d12 d3
-template <class FrP>
-CS_GLOBAL void k_r3_round2_b(R3Round2In in, PlonkConsts K, uint32_t n, int party, PrfArgs P, uint64_t mbase,
+template <class Pol>
+CS_GLOBAL void k_r3_round2_b(R3Round2In in, PlonkConsts K, uint32_t n, int party, typename Pol::Rnd P, uint64_t mbase,
                               const uint32_t* n12, const uint32_t* d12, uint32_t* on, uint32_t* od, uint32_t* pn, uint32_t* pd) {
   uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
-  Sh<FrP> n3, d3;
-  r3_factors<FrP>(in, K, n, i, party, 2, n3, d3);
-  st_reshare<FrP>(on, pn, i, sh_lmul<FrP>(ld_sh<FrP>(n12, i), n3) + prf_mask<FrP>(P, mbase + i));
-  st_reshare<FrP>(od, pd, i, sh_lmul<FrP>(ld_sh<FrP>(d12, i), d3) + prf_mask<FrP>(P, mbase + n + i));
+  typename Pol::S n3, d3;
+  r3_factors<Pol>(in, K, n, i, party, 2, n3, d3);
+  Pol::st_prod(on, pn, i, Pol::masked(Pol::lmul(Pol::ld(n12, i), n3), P, mbase + i));
+  Pol::st_prod(od, pd, i, Pol::masked(Pol::lmul(Pol::ld(d12, i), d3), P, mbase + n + i));
 }
 // masked values to open: g_i = den_i s_i (i < n), q_k = r_k s'_k (k <= n); s, r, s' are fresh random shares
-// drawn from the correlated streams at rbase (s: [0,n), r: [n, 2n+1), s': [2n+1, 3n+2)).  Additive outputs.
-template <class FrP>
-CS_GLOBAL void k_r3_round2_c(const uint32_t* den, uint32_t n, PrfArgs P, uint64_t rbase, uint64_t mbase,
+// (Rep3: drawn from the correlated streams at rbase; s: [0,n), r: [n, 2n+1), s': [2n+1, 3n+2)).  Additive (Rep3) or
+// degree-2t (Shamir) outputs.
+template <class Pol>
+CS_GLOBAL void k_r3_round2_c(const uint32_t* den, uint32_t n, typename Pol::Rnd P, uint64_t rbase, uint64_t mbase,
                               uint32_t* out_g, uint32_t* out_q) {
+  typedef typename Pol::FrP FrP;
   uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i > n) return;
-  Sh<FrP> r = prf_share<FrP>(P, rbase, n + i), sp = prf_share<FrP>(P, rbase, 2 * n + 1 + i);
-  st_fr<FrP>(out_q + (size_t)i * FrP::N, sh_lmul<FrP>(r, sp) + prf_mask<FrP>(P, mbase + n + i));
+  typename Pol::S r = Pol::rand(P, rbase, n + i), sp = Pol::rand(P, rbase, 2 * n + 1 + i);
+  st_fr<FrP>(out_q + (size_t)i * FrP::N, Pol::masked(Pol::lmul(r, sp), P, mbase + n + i));
   if (i < n) {
-    Sh<FrP> s = prf_share<FrP>(P, rbase, i);
-    st_fr<FrP>(out_g + (size_t)i * FrP::N, sh_lmul<FrP>(ld_sh<FrP>(den, i), s) + prf_mask<FrP>(P, mbase + i));
+    typename Pol::S s = Pol::rand(P, rbase, i);
+    st_fr<FrP>(out_g + (size_t)i * FrP::N, Pol::masked(Pol::lmul(Pol::ld(den, i), s), P, mbase + i));
   }
 }
 // with G^-1, Q^-1 public: 1/den_i = s_i / G_i,  x_i = num_i / den_i;  u_{i+1} = (s'_0 / Q_0) r_{i+1}
-template <class FrP>
-CS_GLOBAL void k_r3_round2_d(const uint32_t* num, const uint32_t* ginv, const uint32_t* qinv, uint32_t n, PrfArgs P,
+template <class Pol>
+CS_GLOBAL void k_r3_round2_d(const uint32_t* num, const uint32_t* ginv, const uint32_t* qinv, uint32_t n, typename Pol::Rnd P,
                               uint64_t rbase, uint64_t mbase, uint32_t* ox, uint32_t* ou, uint32_t* px, uint32_t* pu) {
+  typedef typename Pol::FrP FrP;
   uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
   constexpr int NW = FrP::N;
-  Sh<FrP> deninv = sh_mulp<FrP>(prf_share<FrP>(P, rbase, i), ld_fr<FrP>(ginv + (size_t)i * NW));
-  st_reshare<FrP>(ox, px, i, sh_lmul<FrP>(ld_sh<FrP>(num, i), deninv) + prf_mask<FrP>(P, mbase + i));
-  Sh<FrP> rinv0 = sh_mulp<FrP>(prf_share<FrP>(P, rbase, 2 * n + 1), ld_fr<FrP>(qinv));
-  st_reshare<FrP>(ou, pu, i, sh_lmul<FrP>(rinv0, prf_share<FrP>(P, rbase, n + i + 1)) + prf_mask<FrP>(P, mbase + n + i));
+  typename Pol::S deninv = Pol::mulp(Pol::rand(P, rbase, i), ld_fr<FrP>(ginv + (size_t)i * NW));
+  Pol::st_prod(ox, px, i, Pol::masked(Pol::lmul(Pol::ld(num, i), deninv), P, mbase + i));
+  typename Pol::S rinv0 = Pol::mulp(Pol::rand(P, rbase, 2 * n + 1), ld_fr<FrP>(qinv));
+  Pol::st_prod(ou, pu, i, Pol::masked(Pol::lmul(rinv0, Pol::rand(P, rbase, n + i + 1)), P, mbase + n + i));
 }
 // m_i = r_i x_i
-template <class FrP>
-CS_GLOBAL void k_r3_round2_e(const uint32_t* x, uint32_t n, PrfArgs P, uint64_t rbase, uint64_t mbase, uint32_t* om, uint32_t* pm) {
+template <class Pol>
+CS_GLOBAL void k_r3_round2_e(const uint32_t* x, uint32_t n, typename Pol::Rnd P, uint64_t rbase, uint64_t mbase, uint32_t* om,
+                              uint32_t* pm) {
   uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
-  st_reshare<FrP>(om, pm, i, sh_lmul<FrP>(prf_share<FrP>(P, rbase, n + i), ld_sh<FrP>(x, i)) + prf_mask<FrP>(P, mbase + i));
+  Pol::st_prod(om, pm, i, Pol::masked(Pol::lmul(Pol::rand(P, rbase, n + i), Pol::ld(x, i)), P, mbase + i));
 }
-// y_i = m_i / r_{i+1} = m_i (s'_{i+1} / Q_{i+1}), additive, to be opened
-template <class FrP>
-CS_GLOBAL void k_r3_round2_f(const uint32_t* m, const uint32_t* qinv, uint32_t n, PrfArgs P, uint64_t rbase, uint64_t mbase,
-                              uint32_t* out_y) {
+// y_i = m_i / r_{i+1} = m_i (s'_{i+1} / Q_{i+1}), to be opened
+template <class Pol>
+CS_GLOBAL void k_r3_round2_f(const uint32_t* m, const uint32_t* qinv, uint32_t n, typename Pol::Rnd P, uint64_t rbase,
+                              uint64_t mbase, uint32_t* out_y) {
+  typedef typename Pol::FrP FrP;
   uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
-  Sh<FrP> rinv = sh_mulp<FrP>(prf_share<FrP>(P, rbase, 2 * n + 1 + i + 1), ld_fr<FrP>(qinv + (size_t)(i + 1) * FrP::N));
-  st_fr<FrP>(out_y + (size_t)i * FrP::N, sh_lmul<FrP>(ld_sh<FrP>(m, i), rinv) + prf_mask<FrP>(P, mbase + i));
+  typename Pol::S rinv = Pol::mulp(Pol::rand(P, rbase, 2 * n + 1 + i + 1), ld_fr<FrP>(qinv + (size_t)(i + 1) * FrP::N));
+  st_fr<FrP>(out_y + (size_t)i * FrP::N, Pol::masked(Pol::lmul(Pol::ld(m, i), rinv), P, mbase + i));
 }
 // prod_{j<=i} x_j = Y_0..Y_i * u_{i+1}  (Y public running products);  buffer_z is that rotated right by one
-template <class FrP>
+template <class Pol>
 CS_GLOBAL void k_r3_round2_g(const uint32_t* ypref, const uint32_t* u, uint32_t n, uint32_t* zbuf) {
+  typedef typename Pol::FrP FrP;
   uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
-  st_sh<FrP>(zbuf, (i + 1) % n, sh_mulp<FrP>(ld_sh<FrP>(u, i), ld_fr<FrP>(ypref + (size_t)i * FrP::N)));
+  Pol::st(zbuf, (i + 1) % n, Pol::mulp(Pol::ld(u, i), ld_fr<FrP>(ypref + (size_t)i * FrP::N)));
 }
 
 // elementwise inverse of a public vector from its prefix / suffix products and 1/total
@@ -182,127 +241,132 @@ struct R3QuotIn {
   const uint32_t* tw4;
 };
 struct R3Blinders { ShConst b[9]; };
-template <class FrP>
+template <class Pol>
 struct R3Point {
-  Sh<FrP> a, b, c, z, zw, ap, bp, cp, zp, zwp;
-  Fp<FrP> w;
+  typename Pol::S a, b, c, z, zw, ap, bp, cp, zp, zwp;
+  Fp<typename Pol::FrP> w;
 };
-template <class FrP>
-CS_D R3Point<FrP> r3_point(const R3QuotIn& in, const R3Blinders& B, uint32_t n, uint32_t i) {
+template <class Pol>
+CS_D R3Point<Pol> r3_point(const R3QuotIn& in, const R3Blinders& B, uint32_t n, uint32_t i) {
+  typedef typename Pol::FrP FrP;
   typedef Fp<FrP> F;
   const uint32_t n4 = 4 * n;
-  R3Point<FrP> p;
+  R3Point<Pol> p;
   p.w = root_pow<FrP>(in.tw4, 2 * n, i);
   F ww = root_pow<FrP>(in.tw4, 2 * n, (i + 4) % n4);
-  p.a = ld_sh<FrP>(in.a, i); p.b = ld_sh<FrP>(in.b, i); p.c = ld_sh<FrP>(in.c, i); p.z = ld_sh<FrP>(in.z, i);
-  p.zw = ld_sh<FrP>(in.z, (i + 4) % n4);
-  p.ap = sh_add<FrP>(sh_const<FrP>(B.b[1]), sh_mulp<FrP>(sh_const<FrP>(B.b[0]), p.w));
-  p.bp = sh_add<FrP>(sh_const<FrP>(B.b[3]), sh_mulp<FrP>(sh_const<FrP>(B.b[2]), p.w));
-  p.cp = sh_add<FrP>(sh_const<FrP>(B.b[5]), sh_mulp<FrP>(sh_const<FrP>(B.b[4]), p.w));
-  Sh<FrP> b6 = sh_const<FrP>(B.b[6]), b7 = sh_const<FrP>(B.b[7]), b8 = sh_const<FrP>(B.b[8]);
-  p.zp = sh_add<FrP>(sh_add<FrP>(sh_mulp<FrP>(b6, p.w.sqr()), sh_mulp<FrP>(b7, p.w)), b8);
-  p.zwp = sh_add<FrP>(sh_add<FrP>(sh_mulp<FrP>(b6, ww.sqr()), sh_mulp<FrP>(b7, ww)), b8);
+  p.a = Pol::ld(in.a, i); p.b = Pol::ld(in.b, i); p.c = Pol::ld(in.c, i); p.z = Pol::ld(in.z, i);
+  p.zw = Pol::ld(in.z, (i + 4) % n4);
+  p.ap = Pol::add(Pol::cnst(B.b[1]), Pol::mulp(Pol::cnst(B.b[0]), p.w));
+  p.bp = Pol::add(Pol::cnst(B.b[3]), Pol::mulp(Pol::cnst(B.b[2]), p.w));
+  p.cp = Pol::add(Pol::cnst(B.b[5]), Pol::mulp(Pol::cnst(B.b[4]), p.w));
+  typename Pol::S b6 = Pol::cnst(B.b[6]), b7 = Pol::cnst(B.b[7]), b8 = Pol::cnst(B.b[8]);
+  p.zp = Pol::add(Pol::add(Pol::mulp(b6, p.w.sqr()), Pol::mulp(b7, p.w)), b8);
+  p.zwp = Pol::add(Pol::add(Pol::mulp(b6, ww.sqr()), Pol::mulp(b7, ww)), b8);
   return p;
 }
 // the twelve first-layer products: ab a.bp ap.b ap.bp | cz c.zp cp.z cp.zp | c.zw c.zwp cp.zw cp.zwp
 // slot k of the arena holds product k (4n shares); masks at mbase + k 4n + i
-template <class FrP>
-CS_GLOBAL void k_r3_quot_l1(R3QuotIn in, R3Blinders B, uint32_t n, PrfArgs P, uint64_t mbase, uint32_t* arena, uint32_t* peer,
-                             size_t slot_words) {
+template <class Pol>
+CS_GLOBAL void k_r3_quot_l1(R3QuotIn in, R3Blinders B, uint32_t n, typename Pol::Rnd P, uint64_t mbase, uint32_t* arena,
+                             uint32_t* peer, size_t slot_words) {
+  typedef typename Pol::S S;
   const uint32_t n4 = 4 * n;
   uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n4) return;
-  R3Point<FrP> p = r3_point<FrP>(in, B, n, i);
-  const Sh<FrP>* L[12] = {&p.a, &p.a, &p.ap, &p.ap, &p.c, &p.c, &p.cp, &p.cp, &p.c, &p.c, &p.cp, &p.cp};
-  const Sh<FrP>* R[12] = {&p.b, &p.bp, &p.b, &p.bp, &p.z, &p.zp, &p.z, &p.zp, &p.zw, &p.zwp, &p.zw, &p.zwp};
+  R3Point<Pol> p = r3_point<Pol>(in, B, n, i);
+  const S* L[12] = {&p.a, &p.a, &p.ap, &p.ap, &p.c, &p.c, &p.cp, &p.cp, &p.c, &p.c, &p.cp, &p.cp};
+  const S* R[12] = {&p.b, &p.bp, &p.b, &p.bp, &p.z, &p.zp, &p.z, &p.zp, &p.zw, &p.zwp, &p.zw, &p.zwp};
   for (int k = 0; k < 12; k++)
-    st_reshare<FrP>(arena + (size_t)k * slot_words, peer ? peer + (size_t)k * slot_words : (uint32_t*)nullptr, i,
-                    sh_lmul<FrP>(*L[k], *R[k]) + prf_mask<FrP>(P, mbase + (uint64_t)k * n4 + i));
+    Pol::st_prod(arena + (size_t)k * slot_words, peer ? peer + (size_t)k * slot_words : (uint32_t*)nullptr, i,
+                 Pol::masked(Pol::lmul(*L[k], *R[k]), P, mbase + (uint64_t)k * n4 + i));
 }
 
 struct R3KeyEvals {
   const uint32_t *qm, *ql, *qr, *qo, *qc, *s1, *s2, *s3, *lagrange, *buf_a;  // buf_a: n shares
 };
-// e = (A)(B)(C)(D) with blinding parts, from the four (a,b)-type and four (c,d)-type products (replicated):
-// value r and, for m != 0, the Z_H-weighted blinding sum (mul4vec / mul4vec_post, round3.rs:20-108), additive
-template <class FrP>
-CS_D void r3_mul4(const Sh<FrP>& ab, const Sh<FrP>& abp, const Sh<FrP>& apb, const Sh<FrP>& apbp, const Sh<FrP>& cd,
-                  const Sh<FrP>& cdp, const Sh<FrP>& cpd, const Sh<FrP>& cpdp, uint32_t m, const PlonkConsts& K, Fp<FrP>& r,
-                  Fp<FrP>& rz) {
-  Sh<FrP> s1 = sh_add<FrP>(apb, abp), s2 = sh_add<FrP>(cpd, cdp);
-  r = sh_lmul<FrP>(ab, cd);
-  rz = sh_lmul<FrP>(s1, cd) + sh_lmul<FrP>(ab, s2);
+// e = (A)(B)(C)(D) with blinding parts, from the four (a,b)-type and four (c,d)-type products:
+// value r and, for m != 0, the Z_H-weighted blinding sum (mul4vec / mul4vec_post, round3.rs:20-108)
+template <class Pol>
+CS_D void r3_mul4(const typename Pol::S& ab, const typename Pol::S& abp, const typename Pol::S& apb, const typename Pol::S& apbp,
+                  const typename Pol::S& cd, const typename Pol::S& cdp, const typename Pol::S& cpd, const typename Pol::S& cpdp,
+                  uint32_t m, const PlonkConsts& K, Fp<typename Pol::FrP>& r, Fp<typename Pol::FrP>& rz) {
+  typedef typename Pol::FrP FrP;
+  typename Pol::S s1 = Pol::add(apb, abp), s2 = Pol::add(cpd, cdp);
+  r = Pol::lmul(ab, cd);
+  rz = Pol::lmul(s1, cd) + Pol::lmul(ab, s2);
   if (m) {
-    Fp<FrP> x1 = sh_lmul<FrP>(apbp, cd) + sh_lmul<FrP>(s1, s2) + sh_lmul<FrP>(ab, cpdp);
-    Fp<FrP> x2 = sh_lmul<FrP>(s1, cpdp) + sh_lmul<FrP>(apbp, s2);
-    Fp<FrP> x3 = sh_lmul<FrP>(apbp, cpdp);
+    Fp<FrP> x1 = Pol::lmul(apbp, cd) + Pol::lmul(s1, s2) + Pol::lmul(ab, cpdp);
+    Fp<FrP> x2 = Pol::lmul(s1, cpdp) + Pol::lmul(apbp, s2);
+    Fp<FrP> x3 = Pol::lmul(apbp, cpdp);
     rz = rz + x1 * cload<FrP>(K.z1[m]) + x2 * cload<FrP>(K.z2[m]) + x3 * cload<FrP>(K.z3[m]);
   }
 }
-// layer 2: additive shares of t and tz at every extended-domain point (compute_t, round3.rs:300-520).
+// layer 2: t and tz at every extended-domain point (compute_t, round3.rs:300-520) -- additive shares (Rep3) or
+// degree-2t shares (Shamir).
 // Operands are fetched where they are used (first-layer products from the arena, wire / z evaluations and their
 // blinding parts recomputed from the nine blinders): holding the twelve products and the ten point values at once
 // needed ~350 registers and spilled; the re-reads hit L1/L2.
-template <class FrP>
+template <class Pol>
 CS_GLOBAL void k_r3_quot_l2(R3QuotIn in, R3Blinders B, R3KeyEvals E, uint32_t n, uint32_t nlag, PlonkConsts K, int party,
-                             PrfArgs P, uint64_t mbase, const uint32_t* arena, size_t slot_words, uint32_t* t_out,
+                             typename Pol::Rnd P, uint64_t mbase, const uint32_t* arena, size_t slot_words, uint32_t* t_out,
                              uint32_t* tz_out) {
+  typedef typename Pol::FrP FrP;
   typedef Fp<FrP> F;
-  typedef Sh<FrP> S;
+  typedef typename Pol::S S;
   constexpr int NW = FrP::N;
   const uint32_t n4 = 4 * n;
   uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n4) return;
   const uint32_t m = i & 3;
   const F w = root_pow<FrP>(in.tw4, 2 * n, i);
-  auto PR = [&](int k) { return ld_sh<FrP>(arena + (size_t)k * slot_words, i); };
-  auto lin = [&](int hi, int lo) { return sh_add<FrP>(sh_const<FrP>(B.b[lo]), sh_mulp<FrP>(sh_const<FrP>(B.b[hi]), w)); };
+  auto PR = [&](int k) { return Pol::ld(arena + (size_t)k * slot_words, i); };
+  auto lin = [&](int hi, int lo) { return Pol::add(Pol::cnst(B.b[lo]), Pol::mulp(Pol::cnst(B.b[hi]), w)); };
   auto quad = [&](const F& x) {  // b6 x^2 + b7 x + b8
-    return sh_add<FrP>(sh_add<FrP>(sh_mulp<FrP>(sh_const<FrP>(B.b[6]), x.sqr()), sh_mulp<FrP>(sh_const<FrP>(B.b[7]), x)), sh_const<FrP>(B.b[8]));
+    return Pol::add(Pol::add(Pol::mulp(Pol::cnst(B.b[6]), x.sqr()), Pol::mulp(Pol::cnst(B.b[7]), x)), Pol::cnst(B.b[8]));
   };
   const F beta = cload<FrP>(K.beta), gamma = cload<FrP>(K.gamma);
-  // e1, e1z: linear in the first-layer products -> this party's additive part is the .a component
+  // e1, e1z: linear in the first-layer products -> this party's part of them (Rep3: the .a component)
   F e1, e1z;
   {
     const F qm = ld_fr<FrP>(E.qm + (size_t)i * NW), ql = ld_fr<FrP>(E.ql + (size_t)i * NW), qr = ld_fr<FrP>(E.qr + (size_t)i * NW),
             qo = ld_fr<FrP>(E.qo + (size_t)i * NW);
-    e1 = PR(0).a * qm + ld_sh<FrP>(in.a, i).a * ql + ld_sh<FrP>(in.b, i).a * qr + ld_sh<FrP>(in.c, i).a * qo;
-    F a0 = PR(1).a + PR(2).a;
-    if (m) a0 = a0 + PR(3).a * cload<FrP>(K.z1[m]);
-    e1z = a0 * qm + lin(0, 1).a * ql + lin(2, 3).a * qr + lin(4, 5).a * qo;
+    e1 = Pol::part(PR(0)) * qm + Pol::part(Pol::ld(in.a, i)) * ql + Pol::part(Pol::ld(in.b, i)) * qr + Pol::part(Pol::ld(in.c, i)) * qo;
+    F a0 = Pol::part(PR(1)) + Pol::part(PR(2));
+    if (m) a0 = a0 + Pol::part(PR(3)) * cload<FrP>(K.z1[m]);
+    e1z = a0 * qm + Pol::part(lin(0, 1)) * ql + Pol::part(lin(2, 3)) * qr + Pol::part(lin(4, 5)) * qo;
     for (uint32_t j = 0; j < nlag; j++)
-      e1 = e1 - ld_fr<FrP>(E.buf_a + (size_t)(2 * j) * NW) * ld_fr<FrP>(E.lagrange + ((size_t)j * n4 + i) * NW);
-    if (party == 0) e1 = e1 + ld_fr<FrP>(E.qc + (size_t)i * NW);
+      e1 = e1 - Pol::part(Pol::ld(E.buf_a, j)) * ld_fr<FrP>(E.lagrange + ((size_t)j * n4 + i) * NW);
+    if (Pol::pub(party)) e1 = e1 + ld_fr<FrP>(E.qc + (size_t)i * NW);
   }
   // e2: (a + oa)(b + ob)(c + oc) z with oa = beta w + gamma, ...
   F e2, e2z, e3, e3z;
   {
     const F bw = beta * w;
     const F oa = bw + gamma, ob = bw * cload<FrP>(K.k1) + gamma, oc = bw * cload<FrP>(K.k2) + gamma;
-    S ab = sh_addp<FrP>(sh_add<FrP>(PR(0), sh_add<FrP>(sh_mulp<FrP>(ld_sh<FrP>(in.a, i), ob), sh_mulp<FrP>(ld_sh<FrP>(in.b, i), oa))), oa * ob, party);
-    S abp = sh_add<FrP>(PR(1), sh_mulp<FrP>(lin(2, 3), oa));
-    S apb = sh_add<FrP>(PR(2), sh_mulp<FrP>(lin(0, 1), ob));
-    S cd = sh_add<FrP>(PR(4), sh_mulp<FrP>(ld_sh<FrP>(in.z, i), oc));
-    S cdp = sh_add<FrP>(PR(5), sh_mulp<FrP>(quad(w), oc));
-    r3_mul4<FrP>(ab, abp, apb, PR(3), cd, cdp, PR(6), PR(7), m, K, e2, e2z);
+    S ab = Pol::addp(Pol::add(PR(0), Pol::add(Pol::mulp(Pol::ld(in.a, i), ob), Pol::mulp(Pol::ld(in.b, i), oa))), oa * ob, party);
+    S abp = Pol::add(PR(1), Pol::mulp(lin(2, 3), oa));
+    S apb = Pol::add(PR(2), Pol::mulp(lin(0, 1), ob));
+    S cd = Pol::add(PR(4), Pol::mulp(Pol::ld(in.z, i), oc));
+    S cdp = Pol::add(PR(5), Pol::mulp(quad(w), oc));
+    r3_mul4<Pol>(ab, abp, apb, PR(3), cd, cdp, PR(6), PR(7), m, K, e2, e2z);
   }
   {
     const F o1 = ld_fr<FrP>(E.s1 + (size_t)i * NW) * beta + gamma, o2 = ld_fr<FrP>(E.s2 + (size_t)i * NW) * beta + gamma,
             o3 = ld_fr<FrP>(E.s3 + (size_t)i * NW) * beta + gamma;
-    S ab = sh_addp<FrP>(sh_add<FrP>(PR(0), sh_add<FrP>(sh_mulp<FrP>(ld_sh<FrP>(in.a, i), o2), sh_mulp<FrP>(ld_sh<FrP>(in.b, i), o1))), o1 * o2, party);
-    S abp = sh_add<FrP>(PR(1), sh_mulp<FrP>(lin(2, 3), o1));
-    S apb = sh_add<FrP>(PR(2), sh_mulp<FrP>(lin(0, 1), o2));
-    S cd = sh_add<FrP>(PR(8), sh_mulp<FrP>(ld_sh<FrP>(in.z, (i + 4) % n4), o3));
-    S cdp = sh_add<FrP>(PR(9), sh_mulp<FrP>(quad(root_pow<FrP>(in.tw4, 2 * n, (i + 4) % n4)), o3));
-    r3_mul4<FrP>(ab, abp, apb, PR(3), cd, cdp, PR(10), PR(11), m, K, e3, e3z);
+    S ab = Pol::addp(Pol::add(PR(0), Pol::add(Pol::mulp(Pol::ld(in.a, i), o2), Pol::mulp(Pol::ld(in.b, i), o1))), o1 * o2, party);
+    S abp = Pol::add(PR(1), Pol::mulp(lin(2, 3), o1));
+    S apb = Pol::add(PR(2), Pol::mulp(lin(0, 1), o2));
+    S cd = Pol::add(PR(8), Pol::mulp(Pol::ld(in.z, (i + 4) % n4), o3));
+    S cdp = Pol::add(PR(9), Pol::mulp(quad(root_pow<FrP>(in.tw4, 2 * n, (i + 4) % n4)), o3));
+    r3_mul4<Pol>(ab, abp, apb, PR(3), cd, cdp, PR(10), PR(11), m, K, e3, e3z);
   }
   const F alpha = cload<FrP>(K.alpha);
   const F l0a2 = ld_fr<FrP>(E.lagrange + (size_t)i * NW) * cload<FrP>(K.alpha2);
-  F zm1 = ld_sh<FrP>(in.z, i).a;
-  if (party == 0) zm1 = zm1 - F::one();
-  const F e4 = zm1 * l0a2, e4z = quad(w).a * l0a2;
-  st_fr<FrP>(t_out + (size_t)i * NW, e1 + (e2 - e3) * alpha + e4 + prf_mask<FrP>(P, mbase + i));
-  st_fr<FrP>(tz_out + (size_t)i * NW, e1z + (e2z - e3z) * alpha + e4z + prf_mask<FrP>(P, mbase + n4 + i));
+  F zm1 = Pol::part(Pol::ld(in.z, i));
+  if (Pol::pub(party)) zm1 = zm1 - F::one();
+  const F e4 = zm1 * l0a2, e4z = Pol::part(quad(w)) * l0a2;
+  st_fr<FrP>(t_out + (size_t)i * NW, Pol::masked(e1 + (e2 - e3) * alpha + e4, P, mbase + i));
+  st_fr<FrP>(tz_out + (size_t)i * NW, Pol::masked(e1z + (e2z - e3z) * alpha + e4z, P, mbase + n4 + i));
 }
 
 }  // namespace cs

@@ -11,8 +11,15 @@
 // pairwise PRG seeds (t parties derive their shares locally); here every dealer sends every share explicitly.  The
 // resulting objects -- t + 1 uniformly random double sharings per batch, extracted with the (t+1) x n Vandermonde
 // matrix -- are the same, only the preprocessing traffic is larger (2 field elements per pair and recipient).
+//
+// Plonk-sized consumers (cs_plonk_shamir) take their pairs from the device: shamir_double_sharings deals, exchanges and
+// extracts whole vectors of pairs with k_fr_rand and k_vec_lincomb (no host arithmetic per pair), and
+// shamir_degree_reduce / shamir_open_vec work on device vectors.  The host pair pool below stays for point-sized
+// consumers (degree_reduce_point, cs_shamir_state_rand).
+#include <algorithm>
 #include "cs_lib.cuh"
 #include "cs_net.h"
+#include "cs_shamir.cuh"
 
 using namespace cs;
 
@@ -23,6 +30,7 @@ struct cs_shamir_state {
   std::vector<uint64_t> r_t, r_2t;  // buffered pairs
   size_t generation_amount = 1024;  // ShamirState::DEFAULT_PAIR_GEN_AMOUNT, doubled on every refill
   HostChaCha rng;
+  ShamirWorkspace ws;  // staging of the vector routines, kept between calls
 };
 
 namespace {
@@ -225,9 +233,10 @@ int degree_reduce_point_t(cs_shamir_state* st, cs_net* net, const uint64_t* base
   return 0;
 }
 
-// open_half_point (pointshare.rs:102-111): broadcast_next over 2t + 1 parties, Lagrange-weighted sum
+// open_point_many (pointshare.rs:129) / open_half_point (:102-111): broadcast_next over d + 1 parties (d = t or 2t),
+// Lagrange-weighted sum, for `k` points in place
 template <class Cfg, int G>
-int open_half_point_t(cs_shamir_state* st, cs_net* net, const uint64_t* in, uint64_t* out) {
+int open_points_t(cs_shamir_state* st, cs_net* net, int degree_2t, uint64_t* pts, size_t k) {
   typedef typename GroupOf<Cfg, G>::HF HF;
   typedef host::HXyzz<HF> X;
   typedef host::HAffine<HF> A;
@@ -235,20 +244,245 @@ int open_half_point_t(cs_shamir_state* st, cs_net* net, const uint64_t* in, uint
   const size_t PL = sizeof(A) / 8;
   auto load = [](const uint64_t* p) { A a; memcpy(&a, p, sizeof(a)); return X::from_affine(a); };
   auto mul_mont = [](const X& p, const uint64_t* s) { HR v; memcpy(v.l, s, sizeof(v.l)); HR c = v.from_mont(); return host::hmul(p, c.l, HR::N); };
-  const int n = st->n, num = 2 * st->t + 1, id = st->id;
-  for (int s = 1; s < num; s++) CS_TRY(cs_net_send(net, (id + s) % n, in, PL * 8));
-  X acc = mul_mont(load(in), &st->open_lagrange_2t[0]);
-  std::vector<uint64_t> buf(PL);
+  const int n = st->n, num = (degree_2t ? 2 * st->t : st->t) + 1, id = st->id;
+  const std::vector<uint64_t>& lag = degree_2t ? st->open_lagrange_2t : st->open_lagrange_t;
+  for (int s = 1; s < num; s++) CS_TRY(cs_net_send(net, (id + s) % n, pts, k * PL * 8));
+  std::vector<X> acc(k);
+  for (size_t i = 0; i < k; i++) acc[i] = mul_mont(load(pts + i * PL), &lag[0]);
+  std::vector<uint64_t> buf(k * PL);
   for (int r = 1; r < num; r++) {
-    CS_TRY(cs_net_recv(net, (id + n - r) % n, buf.data(), PL * 8));
-    acc = host::hadd(acc, mul_mont(load(buf.data()), &st->open_lagrange_2t[4 * r]));
+    CS_TRY(cs_net_recv(net, (id + n - r) % n, buf.data(), k * PL * 8));
+    for (size_t i = 0; i < k; i++) acc[i] = host::hadd(acc[i], mul_mont(load(buf.data() + i * PL), &lag[4 * r]));
   }
-  A a = host::haffine(acc);
-  memcpy(out, &a, sizeof(a));
+  for (size_t i = 0; i < k; i++) {
+    A a = host::haffine(acc[i]);
+    memcpy(pts + i * PL, &a, sizeof(a));
+  }
   return 0;
 }
 
 }  // namespace
+
+namespace cs {
+
+// Batches (t + 1 pairs each) per dealing round: bounds the device and host staging of one round to ~(3t + 2n + 3)
+// x 32 MB and makes every round take a fresh seed.
+constexpr size_t PAIR_BATCHES_MAX = (size_t)1 << 20;
+
+// random_double_share + buffer_triples (rngs.rs:334-470) on device vectors.  Coefficient vectors, structure of arrays
+// over the B batches of a round: [0] s, [1..t] f_1..f_t, [t+1..3t] g_1..g_2t, so that f = s + f_1 x + ... and
+// g = s + g_1 x + ... share their constant term.  Dealing at x = j + 1 is one k_vec_lincomb per degree, the
+// extraction one per Vandermonde row; pair (row, k) lands at index row B + k of the round's output range.
+int shamir_double_sharings(cs_ctx* ctx, cs_shamir_state* st, cs_net* net, size_t count, uint64_t* d_rt, uint64_t* d_r2t) {
+  if (count == 0) return 0;
+  const int n = st->n, t = st->t, id = st->id;
+  if (n > (int)LINCOMB_MAX) return fail(CS_ERR_LIMIT, "shamir_double_sharings: %d parties exceed %u", n, LINCOMB_MAX);
+  const cs_curve cv = (cs_curve)st->curve;
+  const size_t nc = 3 * (size_t)t + 1;
+  CS_CUDA(cudaSetDevice(ctx->device));
+  const size_t bmax = std::min(PAIR_BATCHES_MAX, (count + t) / (t + 1));
+  ShamirWorkspace& ws = st->ws;
+  DevBuf &coef = ws.coef, &rcv = ws.rcv, &msg = ws.msg;
+  CS_TRY(coef.reserve(nc * bmax * 32));
+  CS_TRY(rcv.reserve(2 * (size_t)n * bmax * 32));
+  CS_TRY(msg.reserve(2 * bmax * 32));
+  uint64_t* hs = ws.host0(2 * bmax * 4);
+  uint64_t* hr = ws.host1(2 * bmax * 4);
+  // w[e] = x^e in Montgomery form, e <= 2t
+  auto powers = [&](uint64_t x, uint64_t* w, int m) {
+    uint64_t c[4] = {x, 0, 0, 0}, xm[4];
+    cs_fr_to_mont(cv, c, xm, 1);
+    const uint64_t one[4] = {1, 0, 0, 0};
+    cs_fr_to_mont(cv, one, w, 1);
+    for (int e = 1; e < m; e++) cs_fr_mul(cv, w + 4 * (e - 1), xm, w + 4 * e);
+  };
+  auto cvec = [&](size_t j, size_t B) { return coef.as<uint64_t>() + j * B * 4; };
+  for (size_t done = 0; done < count;) {
+    const size_t todo = std::min(count - done, (size_t)(t + 1) * bmax);
+    const size_t B = (todo + t) / (t + 1);
+    uint8_t seed[32];
+    st->rng.gen_seed(seed);  // one seed per dealing round, never reused
+    CS_TRY(cs_fr_rand_device(ctx, cv, seed, 0, coef.as<uint64_t>(), nc * B));
+    auto deal = [&](int j, uint64_t* out_t, uint64_t* out_2t) -> int {  // f(j + 1), g(j + 1)
+      uint64_t w[4 * LINCOMB_MAX];
+      powers((uint64_t)j + 1, w, 2 * t + 1);
+      const uint64_t* in[LINCOMB_MAX];
+      for (int d = 0; d <= t; d++) in[d] = cvec(d, B);
+      CS_TRY(cs_vec_lincomb(ctx, cv, in, w, t + 1, B, out_t));
+      for (int d = 1; d <= 2 * t; d++) in[d] = cvec(t + d, B);
+      return cs_vec_lincomb(ctx, cv, in, w, 2 * t + 1, B, out_2t);
+    };
+    auto rt_of = [&](int src) { return rcv.as<uint64_t>() + (size_t)src * B * 4; };
+    auto r2t_of = [&](int src) { return rcv.as<uint64_t>() + (size_t)(n + src) * B * 4; };
+    CS_TRY(deal(id, rt_of(id), r2t_of(id)));
+    // all-to-all in n - 1 rounds: round k sends my dealing to party id + k and takes party id - k's
+    for (int round = 1; round < n; round++) {
+      const int j = (id + round) % n, src = (id + n - round) % n;
+      CS_TRY(deal(j, msg.as<uint64_t>(), msg.as<uint64_t>() + B * 4));
+      CS_CUDA(cudaMemcpyAsync(hs, msg.p, 2 * B * 32, cudaMemcpyDeviceToHost, ctx->stream));
+      CS_CUDA(cudaStreamSynchronize(ctx->stream));
+      CS_TRY(cs_net_sendrecv(net, j, hs, 2 * B * 32, src, hr, 2 * B * 32));
+      CS_CUDA(cudaMemcpyAsync(rt_of(src), hr, B * 32, cudaMemcpyHostToDevice, ctx->stream));
+      CS_CUDA(cudaMemcpyAsync(r2t_of(src), hr + B * 4, B * 32, cudaMemcpyHostToDevice, ctx->stream));
+      CS_CUDA(cudaStreamSynchronize(ctx->stream));  // hr is reused by the next round
+    }
+    // DN07 extraction with the (t + 1) x n Vandermonde matrix M[row][col] = (col + 1)^row  (rngs.rs:140-157)
+    for (int row = 0; row <= t; row++) {
+      const size_t lo = (size_t)row * B;
+      if (lo >= todo) break;
+      const size_t len = std::min(B, todo - lo);
+      uint64_t w[4 * LINCOMB_MAX];
+      const uint64_t* in_t[LINCOMB_MAX];
+      const uint64_t* in_2t[LINCOMB_MAX];
+      for (int col = 0; col < n; col++) {
+        uint64_t p[4 * (2 * LINCOMB_MAX)];
+        powers((uint64_t)col + 1, p, row + 1);
+        memcpy(w + 4 * col, p + 4 * row, 32);
+        in_t[col] = rt_of(col);
+        in_2t[col] = r2t_of(col);
+      }
+      CS_TRY(cs_vec_lincomb(ctx, cv, in_t, w, n, len, d_rt + (done + lo) * 4));
+      CS_TRY(cs_vec_lincomb(ctx, cv, in_2t, w, n, len, d_r2t + (done + lo) * 4));
+    }
+    done += todo;
+  }
+  CS_CUDA(cudaStreamSynchronize(ctx->stream));
+  return 0;
+}
+
+// degree_reduce_many (network.rs:150-243): inp += r_2t; parties 1..2t send to the king (party 0), which accumulates
+// with the Lagrange weights (one k_vec_lincomb launch, k = 2t + 1), shares the result as a known polynomial with t zero
+// shares and sends acc * P(id + 1) to parties 0..n-t-1; share -= r_t.
+int shamir_degree_reduce(cs_ctx* ctx, cs_shamir_state* st, cs_net* net, const uint64_t* d_in, size_t len, uint64_t* d_out,
+                         const uint64_t* d_rt, uint64_t* d_r2t) {
+  if (len == 0) return 0;
+  const int n = st->n, t = st->t, id = st->id, num_non_zero = n - t;
+  CS_CUDA(cudaSetDevice(ctx->device));
+  const cs_curve cv = (cs_curve)st->curve;
+  DevBuf* d_stage = st->ws.stage;
+  // inp += r_2t
+  CS_TRY(cs_vec_add(ctx, cv, d_in, d_r2t, d_out, len));
+  uint64_t* host = st->ws.host0(len * 4);
+  int rc = 0;
+  if (id == KING_ID) {
+    // acc = sum_j lagrange_j * inputs_j over parties 0..2t: one k_vec_lincomb launch with k = 2t + 1
+    const uint64_t* ins[LINCOMB_MAX];
+    ins[0] = d_out;
+    for (int other = 1; other <= 2 * t && !rc; other++) {
+      rc = cs_net_recv(net, other, host, len * 32);
+      if (rc) break;
+      rc = d_stage[other].reserve(len * 32);
+      if (rc) break;
+      CS_CUDA(cudaMemcpyAsync(d_stage[other].p, host, len * 32, cudaMemcpyHostToDevice, ctx->stream));
+      CS_CUDA(cudaStreamSynchronize(ctx->stream));  // `host` is reused for the next party
+      ins[other] = d_stage[other].as<uint64_t>();
+    }
+    DevBuf& d_acc = st->ws.acc;
+    if (!rc) rc = d_acc.reserve(len * 32);
+    if (!rc) rc = cs_vec_lincomb(ctx, cv, ins, st->mul_lagrange_2t.data(), 2 * t + 1, len, d_acc.as<uint64_t>());
+    // fresh shares: poly = acc * precomputed, share_id = acc * P(id + 1) -- one scalar per recipient
+    for (int rid = 0; rid < num_non_zero && !rc; rid++) {
+      uint64_t c[4];
+      {
+        const size_t plen = st->mul_reconstruct_with_zeros.size() / 4;
+        // Horner in Fr on the host through the ABI's scalar helpers
+        memcpy(c, &st->mul_reconstruct_with_zeros[4 * (plen - 1)], 32);
+        uint64_t x_can[4] = {(uint64_t)rid + 1, 0, 0, 0}, x[4];
+        cs_fr_to_mont(cv, x_can, x, 1);
+        for (size_t k = plen - 1; k-- > 0;) {
+          cs_fr_mul(cv, c, x, c);
+          cs_fr_add(cv, c, &st->mul_reconstruct_with_zeros[4 * k], c);
+        }
+      }
+      const uint64_t* one_in[1] = {d_acc.as<uint64_t>()};
+      uint64_t* dst = rid == id ? d_out : d_r2t;  // r_2t is no longer needed: reuse as staging
+      rc = cs_vec_lincomb(ctx, cv, one_in, c, 1, len, dst);
+      if (rc || rid == id) continue;
+      CS_CUDA(cudaMemcpyAsync(host, dst, len * 32, cudaMemcpyDeviceToHost, ctx->stream));
+      CS_CUDA(cudaStreamSynchronize(ctx->stream));
+      rc = cs_net_send(net, rid, host, len * 32);
+    }
+  } else {
+    if (id <= 2 * t) {  // only send if my items are required
+      CS_CUDA(cudaMemcpyAsync(host, d_out, len * 32, cudaMemcpyDeviceToHost, ctx->stream));
+      CS_CUDA(cudaStreamSynchronize(ctx->stream));
+      rc = cs_net_send(net, KING_ID, host, len * 32);
+    }
+    if (!rc) {
+      if (id < num_non_zero) {
+        rc = cs_net_recv(net, KING_ID, host, len * 32);
+        if (!rc) CS_CUDA(cudaMemcpyAsync(d_out, host, len * 32, cudaMemcpyHostToDevice, ctx->stream));
+      } else {
+        CS_CUDA(cudaMemsetAsync(d_out, 0, len * 32, ctx->stream));
+      }
+    }
+  }
+  // share -= r_t
+  if (!rc) rc = cs_vec_sub(ctx, cv, d_out, d_rt, d_out, len);
+  if (!rc) CS_CUDA(cudaStreamSynchronize(ctx->stream));
+  return rc;
+}
+
+// open_vec (shamir/arithmetic.rs:191) on a device vector: my shares go to the next d parties, the previous d parties'
+// arrive (one sendrecv per distance, so vectors larger than the mailbox credit window cannot dead-lock), and the
+// Lagrange sum is one k_vec_lincomb launch with k = d + 1.  mul_open_vec (:262) is a local product kernel, then this.
+int shamir_open_vec(cs_ctx* ctx, cs_shamir_state* st, cs_net* net, int degree_2t, const uint64_t* d_in, size_t len, uint64_t* d_out) {
+  if (len == 0) return 0;
+  const int n = st->n, id = st->id, d = degree_2t ? 2 * st->t : st->t;
+  const cs_curve cv = (cs_curve)st->curve;
+  CS_CUDA(cudaSetDevice(ctx->device));
+  uint64_t* mine = st->ws.host0(len * 4);
+  uint64_t* rcv = st->ws.host1(len * 4);
+  CS_CUDA(cudaMemcpyAsync(mine, d_in, len * 32, cudaMemcpyDeviceToHost, ctx->stream));
+  CS_CUDA(cudaStreamSynchronize(ctx->stream));
+  DevBuf* stage = st->ws.stage;
+  const uint64_t* ins[LINCOMB_MAX];
+  ins[0] = d_in;
+  int rc = 0;
+  for (int r = 1; r <= d && !rc; r++) {
+    rc = cs_net_sendrecv(net, (id + r) % n, mine, len * 32, (id + n - r) % n, rcv, len * 32);
+    if (!rc) rc = stage[r].reserve(len * 32);
+    if (rc) break;
+    CS_CUDA(cudaMemcpyAsync(stage[r].p, rcv, len * 32, cudaMemcpyHostToDevice, ctx->stream));
+    CS_CUDA(cudaStreamSynchronize(ctx->stream));  // rcv is reused
+    ins[r] = stage[r].as<uint64_t>();
+  }
+  const std::vector<uint64_t>& lag = degree_2t ? st->open_lagrange_2t : st->open_lagrange_t;
+  if (!rc) rc = cs_vec_lincomb(ctx, cv, ins, lag.data(), d + 1, len, d_out);
+  if (!rc) CS_CUDA(cudaStreamSynchronize(ctx->stream));
+  return rc;
+}
+
+// open_vec on a handful of scalars (host)
+int shamir_open_scalars(cs_shamir_state* st, cs_net* net, int degree_2t, uint64_t* v, size_t k) {
+  const int n = st->n, id = st->id, d = degree_2t ? 2 * st->t : st->t;
+  const cs_curve cv = (cs_curve)st->curve;
+  const std::vector<uint64_t>& lag = degree_2t ? st->open_lagrange_2t : st->open_lagrange_t;
+  for (int s = 1; s <= d; s++) CS_TRY(cs_net_send(net, (id + s) % n, v, k * 32));
+  std::vector<uint64_t> acc(k * 4), buf(k * 4), term(4);
+  for (size_t i = 0; i < k; i++) CS_TRY(cs_fr_mul(cv, v + 4 * i, &lag[0], &acc[4 * i]));
+  for (int r = 1; r <= d; r++) {
+    CS_TRY(cs_net_recv(net, (id + n - r) % n, buf.data(), k * 32));
+    for (size_t i = 0; i < k; i++) {
+      CS_TRY(cs_fr_mul(cv, &buf[4 * i], &lag[4 * r], term.data()));
+      CS_TRY(cs_fr_add(cv, &acc[4 * i], term.data(), &acc[4 * i]));
+    }
+  }
+  memcpy(v, acc.data(), k * 32);
+  return 0;
+}
+
+int shamir_open_points(cs_shamir_state* st, cs_net* net, cs_group group, int degree_2t, uint64_t* pts, size_t k) {
+  CS_DISPATCH_CURVE(st->curve, {
+    if (group == CS_G1) return open_points_t<Cfg, 0>(st, net, degree_2t, pts, k);
+    return open_points_t<Cfg, 1>(st, net, degree_2t, pts, k);
+  });
+  return 0;
+}
+
+size_t shamir_state_device_bytes(const cs_shamir_state* st) { return st ? st->ws.device_bytes() : 0; }
+
+}  // namespace cs
 
 extern "C" {
 
@@ -309,85 +543,27 @@ int cs_shamir_open_lagrange(const cs_shamir_state* st, int degree_2t, uint64_t* 
   return 0;
 }
 
-// degree_reduce_many (network.rs:150-243) on a device-resident vector of degree-2t values.
+// degree_reduce_many (network.rs:150-243) on a device-resident vector of degree-2t values, pairs uploaded from the
+// host pool in the order get_pair hands them out; the reduction itself is shamir_degree_reduce.
 int cs_shamir_degree_reduce_many(cs_ctx* ctx, cs_shamir_state* st, cs_net* net, const uint64_t* d_in, size_t len, uint64_t* d_out) {
   if (!ctx || !st || !net || (len && (!d_in || !d_out))) return fail(CS_ERR_ARG, "cs_shamir_degree_reduce_many: NULL argument");
   if (len == 0) return 0;
-  const int n = st->n, t = st->t, id = st->id, num_non_zero = n - t;
   CS_CUDA(cudaSetDevice(ctx->device));
-  const cs_curve cv = (cs_curve)st->curve;
-  // the pairs this call consumes, in the order get_pair hands them out
   std::vector<uint64_t> rt(len * 4), r2t(len * 4);
   for (size_t i = 0; i < len; i++) CS_TRY(get_pair(st, net, &rt[4 * i], &r2t[4 * i]));
-  DevBuf d_rt, d_r2t, d_stage[LINCOMB_MAX];
+  ScopedBuf d_rt, d_r2t;
   CS_TRY(d_rt.reserve(len * 32));
   CS_TRY(d_r2t.reserve(len * 32));
   CS_CUDA(cudaMemcpyAsync(d_rt.p, rt.data(), len * 32, cudaMemcpyHostToDevice, ctx->stream));
   CS_CUDA(cudaMemcpyAsync(d_r2t.p, r2t.data(), len * 32, cudaMemcpyHostToDevice, ctx->stream));
-  // inp += r_2t
-  CS_TRY(cs_vec_add(ctx, cv, d_in, d_r2t.as<uint64_t>(), d_out, len));
-  std::vector<uint64_t> host(len * 4);
-  auto release = [&]() { d_rt.release(); d_r2t.release(); for (auto& b : d_stage) b.release(); };
-  int rc = 0;
-  if (id == KING_ID) {
-    // acc = sum_j lagrange_j * inputs_j over parties 0..2t: one k_vec_lincomb launch with k = 2t + 1
-    const uint64_t* ins[LINCOMB_MAX];
-    ins[0] = d_out;
-    for (int other = 1; other <= 2 * t && !rc; other++) {
-      rc = cs_net_recv(net, other, host.data(), len * 32);
-      if (rc) break;
-      rc = d_stage[other].reserve(len * 32);
-      if (rc) break;
-      CS_CUDA(cudaMemcpyAsync(d_stage[other].p, host.data(), len * 32, cudaMemcpyHostToDevice, ctx->stream));
-      CS_CUDA(cudaStreamSynchronize(ctx->stream));  // `host` is reused for the next party
-      ins[other] = d_stage[other].as<uint64_t>();
-    }
-    DevBuf d_acc;
-    if (!rc) rc = d_acc.reserve(len * 32);
-    if (!rc) rc = cs_vec_lincomb(ctx, cv, ins, st->mul_lagrange_2t.data(), 2 * t + 1, len, d_acc.as<uint64_t>());
-    // fresh shares: poly = acc * precomputed, share_id = acc * P(id + 1) -- one scalar per recipient
-    for (int rid = 0; rid < num_non_zero && !rc; rid++) {
-      uint64_t c[4];
-      {
-        const size_t plen = st->mul_reconstruct_with_zeros.size() / 4;
-        // Horner in Fr on the host through the ABI's scalar helpers
-        memcpy(c, &st->mul_reconstruct_with_zeros[4 * (plen - 1)], 32);
-        uint64_t x_can[4] = {(uint64_t)rid + 1, 0, 0, 0}, x[4];
-        cs_fr_to_mont(cv, x_can, x, 1);
-        for (size_t k = plen - 1; k-- > 0;) {
-          cs_fr_mul(cv, c, x, c);
-          cs_fr_add(cv, c, &st->mul_reconstruct_with_zeros[4 * k], c);
-        }
-      }
-      const uint64_t* one_in[1] = {d_acc.as<uint64_t>()};
-      uint64_t* dst = rid == id ? d_out : (uint64_t*)d_r2t.p;  // r_2t is no longer needed: reuse as staging
-      rc = cs_vec_lincomb(ctx, cv, one_in, c, 1, len, dst);
-      if (rc || rid == id) continue;
-      CS_CUDA(cudaMemcpyAsync(host.data(), dst, len * 32, cudaMemcpyDeviceToHost, ctx->stream));
-      CS_CUDA(cudaStreamSynchronize(ctx->stream));
-      rc = cs_net_send(net, rid, host.data(), len * 32);
-    }
-    d_acc.release();
-  } else {
-    if (id <= 2 * t) {  // only send if my items are required
-      CS_CUDA(cudaMemcpyAsync(host.data(), d_out, len * 32, cudaMemcpyDeviceToHost, ctx->stream));
-      CS_CUDA(cudaStreamSynchronize(ctx->stream));
-      rc = cs_net_send(net, KING_ID, host.data(), len * 32);
-    }
-    if (!rc) {
-      if (id < num_non_zero) {
-        rc = cs_net_recv(net, KING_ID, host.data(), len * 32);
-        if (!rc) CS_CUDA(cudaMemcpyAsync(d_out, host.data(), len * 32, cudaMemcpyHostToDevice, ctx->stream));
-      } else {
-        CS_CUDA(cudaMemsetAsync(d_out, 0, len * 32, ctx->stream));
-      }
-    }
-  }
-  // share -= r_t
-  if (!rc) rc = cs_vec_sub(ctx, cv, d_out, d_rt.as<uint64_t>(), d_out, len);
-  if (!rc) CS_CUDA(cudaStreamSynchronize(ctx->stream));
-  release();
-  return rc;
+  return shamir_degree_reduce(ctx, st, net, d_in, len, d_out, d_rt.as<uint64_t>(), d_r2t.as<uint64_t>());
+}
+
+int cs_shamir_double_sharings(cs_ctx* ctx, cs_shamir_state* st, cs_net* net, size_t count, uint64_t* d_rt, uint64_t* d_r2t) {
+  if (!ctx || !st || !net || (count && (!d_rt || !d_r2t))) return fail(CS_ERR_ARG, "cs_shamir_double_sharings: NULL argument");
+  if (net->n != st->n || net->id != st->id)
+    return fail(CS_ERR_ARG, "cs_shamir_double_sharings: the net is party %d of %d, the state party %d of %d", net->id, net->n, st->id, st->n);
+  return shamir_double_sharings(ctx, st, net, count, d_rt, d_r2t);
 }
 
 int cs_shamir_degree_reduce_point(cs_shamir_state* st, cs_net* net, cs_group group, const uint64_t* base_affine,
@@ -402,11 +578,8 @@ int cs_shamir_degree_reduce_point(cs_shamir_state* st, cs_net* net, cs_group gro
 
 int cs_shamir_open_half_point(cs_shamir_state* st, cs_net* net, cs_group group, const uint64_t* in_affine, uint64_t* out_affine) {
   if (!st || !net || !in_affine || !out_affine) return fail(CS_ERR_ARG, "cs_shamir_open_half_point: NULL argument");
-  CS_DISPATCH_CURVE(st->curve, {
-    if (group == CS_G1) return open_half_point_t<Cfg, 0>(st, net, in_affine, out_affine);
-    return open_half_point_t<Cfg, 1>(st, net, in_affine, out_affine);
-  });
-  return 0;
+  if (out_affine != in_affine) memmove(out_affine, in_affine, point_limbs64(st->curve, group) * 8);
+  return shamir_open_points(st, net, group, 1, out_affine, 1);
 }
 
 }  // extern "C"

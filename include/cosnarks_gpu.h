@@ -469,6 +469,11 @@ int cs_shamir_degree_reduce_many(cs_ctx* ctx, cs_shamir_state* st, cs_net* net, 
  * (the reference uses the group generator) */
 int cs_shamir_degree_reduce_point(cs_shamir_state* st, cs_net* net, cs_group group, const uint64_t* base_affine,
                                   const uint64_t* in_affine, uint64_t* out_affine);
+/* `count` fresh double sharings (r_t, r_2t) made on the device into d_rt, d_r2t (count elements each): the DN07 steps
+ * of the host pool (explicit dealing at 1..n, all-to-all in n - 1 rounds, (t + 1) x n Vandermonde extraction) with
+ * the dealing coefficients drawn by k_fr_rand under a fresh seed from the state's stream; no host arithmetic per pair.
+ * Every party calls it with the same count. */
+int cs_shamir_double_sharings(cs_ctx* ctx, cs_shamir_state* st, cs_net* net, size_t count, uint64_t* d_rt, uint64_t* d_r2t);
 /* open_half_point: broadcast_next over 2t + 1 parties + reconstruct_point with open_lagrange_2t */
 int cs_shamir_open_half_point(cs_shamir_state* st, cs_net* net, cs_group group, const uint64_t* in_affine, uint64_t* out_affine);
 
@@ -598,6 +603,29 @@ int cs_plonk_rep3_connect_io(cs_plonk_rep3* s, void* d_prev_out, void* d_next_ou
 int cs_plonk_rep3_prove(cs_plonk_rep3* s, cs_net* net, cs_rep3_state* state, const uint64_t* h_public_inputs,
                         size_t n_public_inputs, const uint64_t* h_witness_shares, size_t n_witness,
                         const uint64_t* h_blinder_shares, uint64_t* out_points, uint64_t* out_evals);
+/* ---- Shamir co-Plonk (ShamirCoPlonk::prove, co-plonk/src/lib.rs:237-260; driver mpc/shamir.rs) -- one session per
+ * party of a Shamir(num_parties, threshold) sharing; 1 <= t, 2t + 1 <= n <= 8.  The whole proof runs inside the
+ * library over `net` (n parties; net->id must equal `party`).  Shares are one Montgomery Fr element each (degree t).
+ * Linear steps are the plain prover's kernels on shares; each product layer is a local product followed by one device
+ * degree reduction (cs_plonk_rep3.cuh layering); the double sharings the reductions and random shares consume are made
+ * on the device when rounds 2 and 3 start.  Pairs per proof: 58 domain_size + 2, plus the 11 blinder shares drawn with
+ * ShamirState::rand when h_blinder_shares is NULL (58 domain_size + 13); cs_plonk_shamir_pairs = the last proof's
+ * count, cs_plonk_shamir_pair_ms = the wall time its device pair generation took.
+ *   h_witness_shares: n_witness degree-t shares; h_blinder_shares: 11 degree-t shares of b[0..11), or NULL to draw them;
+ *   out_blinder_shares (optional, 11 x Fr): this party's blinder shares.  out_points / out_evals as cs_plonk_prove_plain;
+ *   every party returns the same opened proof, the plain prover's for the blinders the shares reconstruct to. */
+typedef struct cs_plonk_shamir cs_plonk_shamir;
+int cs_plonk_shamir_create(cs_ctx* ctx, cs_plonk_pk* pk, int num_parties, int threshold, int party, cs_plonk_shamir** out);
+void cs_plonk_shamir_free(cs_plonk_shamir* s);
+int cs_plonk_shamir_prove(cs_plonk_shamir* s, cs_net* net, const uint64_t* h_public_inputs, size_t n_public_inputs,
+                          const uint64_t* h_witness_shares, size_t n_witness, const uint64_t* h_blinder_shares,
+                          uint64_t* out_points, uint64_t* out_evals, uint64_t* out_blinder_shares);
+size_t cs_plonk_shamir_pairs(const cs_plonk_shamir* s);
+double cs_plonk_shamir_pair_ms(const cs_plonk_shamir* s);
+/* device memory the session and its Shamir state hold: workspace, pairs and the staging of the reductions and openings.
+ * Buffers only grow and are kept between proofs, so after a proof this is the party's high-water mark outside the
+ * context (MSM workspaces) and the key. */
+size_t cs_plonk_shamir_device_bytes(const cs_plonk_shamir* s);
 /* sha3::Keccak256 of a host buffer (the transcript hash, types.rs:13-14); test hook. */
 int cs_keccak256(const uint8_t* data, size_t len, uint8_t* out32);
 

@@ -1,12 +1,12 @@
-//! `Plonk::plain_prove` and `Rep3CoPlonk::prove` with the signatures of co-plonk
-//! (co-circom/co-plonk/src/lib.rs:222-240, 271-281), executed by the library: the device-resident key is built
-//! once from the snarkjs `.zkey`, a proof is one FFI call (`cs_plonk_prove_plain`) or, for a Rep3 party, one
-//! `cs_plonk_rep3_prove` -- step sequence, Keccak transcript and openings run inside libcosnarks_gpu.so over the
-//! caller's `mpc_net::Network` through the callback transport.  SOURCE ONLY: never compiled (no rustc in the build
+//! `Plonk::plain_prove`, `Rep3CoPlonk::prove` and `ShamirCoPlonk::prove` with the signatures of co-plonk
+//! (co-circom/co-plonk/src/lib.rs:222-260, 271-281), executed by the library: the device-resident key is built
+//! once from the snarkjs `.zkey`, a proof is one FFI call (`cs_plonk_prove_plain`) or, for an MPC party, one
+//! `cs_plonk_rep3_prove` / `cs_plonk_shamir_prove` -- step sequence, Keccak transcript, openings and (Shamir) the
+//! double sharings run inside libcosnarks_gpu.so over the caller's `mpc_net::Network` through the callback transport.  SOURCE ONLY: never compiled (no rustc in the build
 //! image); the same entry points are exercised from C++ (`include/co_plonk.hpp`) and Python in `tests/`.
 use ark_bn254::{Bn254, Fr};
 use circom_types::plonk::PlonkProof;
-use co_circom_types::{Rep3SharedWitness, SharedWitness};
+use co_circom_types::{Rep3SharedWitness, ShamirSharedWitness, SharedWitness};
 use cosnarks_gpu_sys as sys;
 use mpc_net::Network;
 use std::ffi::CString;
@@ -51,10 +51,11 @@ unsafe extern "C" fn recv_cb<N: Network>(u: *mut c_void, from: c_int, data: *mut
     }
 }
 impl<'a, N: Network> NetAdapter<'a, N> {
-    fn new(net: &'a N) -> eyre::Result<Self> {
+    fn new(net: &'a N) -> eyre::Result<Self> { Self::with_parties(net, 3) }
+    fn with_parties(net: &'a N, parties: usize) -> eyre::Result<Self> {
         let cb = sys::cs_net_callbacks { user: net as *const N as *mut c_void, send: send_cb::<N>, recv: recv_cb::<N> };
         let mut h = std::ptr::null_mut();
-        check(unsafe { sys::cs_net_from_callbacks(net.id() as c_int, 3, &cb, &mut h) })?;
+        check(unsafe { sys::cs_net_from_callbacks(net.id() as c_int, parties as c_int, &cb, &mut h) })?;
         Ok(Self { _net: net, h })
     }
 }
@@ -68,6 +69,7 @@ fn proof_from(points: &[[u64; 8]; 9], evals: &[[u64; 4]; 6]) -> PlonkProof<Bn254
 
 pub struct Plonk;
 pub struct Rep3CoPlonk;
+pub struct ShamirCoPlonk;
 
 impl Plonk {
     /// `Plonk::plain_prove(zkey, private_witness)` (lib.rs:271-281); the eleven round-1 blinders are drawn here
@@ -102,6 +104,31 @@ impl Rep3CoPlonk {
                                      pts.as_mut_ptr().cast(), evs.as_mut_ptr().cast())
         };
         unsafe { sys::cs_plonk_rep3_free(sess); sys::cs_rep3_state_free(state) };
+        check(rc)?;
+        Ok(proof_from(&pts, &evs))
+    }
+}
+
+impl ShamirCoPlonk {
+    /// `ShamirCoPlonk::prove(nets, num_parties, threshold, zkey, witness)` (lib.rs:237-260) for this party.  The
+    /// reference's eight networks become the one `net`; instead of preprocessing `222 domain_size + 15` pairs up front,
+    /// the library makes the 58 domain_size + 2 double sharings the proof consumes on the device when rounds 2 and 3
+    /// start, and draws the eleven blinder shares with ShamirState::rand.
+    pub fn prove<N: Network>(net: &N, num_parties: usize, threshold: usize, zkey: &GpuZkey,
+                             witness: ShamirSharedWitness<Fr>) -> eyre::Result<PlonkProof<Bn254>> {
+        zkey.check_lengths(witness.public_inputs.len(), witness.witness.len())?;
+        let adapter = NetAdapter::with_parties(net, num_parties)?;
+        let mut sess = std::ptr::null_mut();
+        check(unsafe {
+            sys::cs_plonk_shamir_create(zkey.ctx, zkey.pk, num_parties as c_int, threshold as c_int, net.id() as c_int, &mut sess)
+        })?;
+        let (mut pts, mut evs) = ([[0u64; 8]; 9], [[0u64; 4]; 6]);
+        let rc = unsafe {
+            sys::cs_plonk_shamir_prove(sess, adapter.h, witness.public_inputs.as_ptr().cast(), witness.public_inputs.len(),
+                                       witness.witness.as_ptr().cast(), witness.witness.len(), std::ptr::null(),
+                                       pts.as_mut_ptr().cast(), evs.as_mut_ptr().cast(), std::ptr::null_mut())
+        };
+        unsafe { sys::cs_plonk_shamir_free(sess) };
         check(rc)?;
         Ok(proof_from(&pts, &evs))
     }

@@ -6,7 +6,7 @@
 use std::os::raw::{c_char, c_int, c_uint, c_void};
 
 macro_rules! opaque { ($($n:ident),*) => { $( #[repr(C)] pub struct $n { _p: [u8; 0] } )* } }
-opaque!(cs_ctx, cs_bases, cs_domain, cs_groth16_pk, cs_plonk_pk, cs_plonk_rep3, cs_net, cs_rep3_state, cs_shamir_state);
+opaque!(cs_ctx, cs_bases, cs_domain, cs_groth16_pk, cs_plonk_pk, cs_plonk_rep3, cs_plonk_shamir, cs_net, cs_rep3_state, cs_shamir_state);
 
 pub const CS_BN254: c_int = 0;
 pub const CS_BLS12_381: c_int = 1;
@@ -136,6 +136,18 @@ extern "C" {
     pub fn cs_plonk_rep3_prove(s: *mut cs_plonk_rep3, net: *mut cs_net, state: *mut cs_rep3_state, public_inputs: *const u64,
                                n_public_inputs: usize, witness_shares: *const u64, n_witness: usize,
                                blinder_shares: *const u64, out_points: *mut u64, out_evals: *mut u64) -> c_int;
+    // --- Shamir co-Plonk: one session per party of a Shamir(n, t) sharing, the whole proof over one cs_net
+    pub fn cs_plonk_shamir_create(ctx: *mut cs_ctx, pk: *mut cs_plonk_pk, num_parties: c_int, threshold: c_int, party: c_int,
+                                  out: *mut *mut cs_plonk_shamir) -> c_int;
+    pub fn cs_plonk_shamir_free(s: *mut cs_plonk_shamir);
+    pub fn cs_plonk_shamir_prove(s: *mut cs_plonk_shamir, net: *mut cs_net, public_inputs: *const u64, n_public_inputs: usize,
+                                 witness_shares: *const u64, n_witness: usize, blinder_shares: *const u64,
+                                 out_points: *mut u64, out_evals: *mut u64, out_blinder_shares: *mut u64) -> c_int;
+    pub fn cs_plonk_shamir_pairs(s: *const cs_plonk_shamir) -> usize;
+    pub fn cs_plonk_shamir_pair_ms(s: *const cs_plonk_shamir) -> f64;
+    pub fn cs_plonk_shamir_device_bytes(s: *const cs_plonk_shamir) -> usize;
+    pub fn cs_shamir_double_sharings(ctx: *mut cs_ctx, st: *mut cs_shamir_state, net: *mut cs_net, count: usize,
+                                     d_rt: *mut u64, d_r2t: *mut u64) -> c_int;
     // --- large-vector Rep3 products, batched VM opcodes, Honk commitments and sumcheck kernels
     pub fn cs_rep3_mul_vec_reshare(ctx: *mut cs_ctx, curve: c_int, d_a: *const u64, d_b: *const u64, n: usize,
                                    prf: *const cs_rep3_prf, d_out: *mut u64, d_next_out: *mut u64) -> c_int;

@@ -1,7 +1,14 @@
 """Rep3 co-Plonk, three parties on three GPUs of one box (products stored into the next party's GPU over NVLink,
 openings over NCCL): wall time per proof, max over ranks, proof checked by the oracle's verifier on rank 0.
 launch: python -m torch.distributed.run --nnodes=1 --nproc-per-node 3 --master-addr 127.0.0.1 --master-port 29519 \
-        tools/time_co_plonk.py [log_n ...]"""
+        tools/time_co_plonk.py [log_n ...]
+
+python tools/time_co_plonk.py --shamir N T [log_n ...]: no torchrun; on cuda:0, three Rep3 party threads and then N
+Shamir(N, T) party threads (cs_plonk_shamir_prove), each over in-process mailbox nets, proofs checked by the oracle's
+verifier.  Per size: ms per proof for both, the Shamir split into device pair generation and the rounds, pairs,
+bytes sent per party, the device's peak memory during a proof above its level at the proof's start, and what each party's
+session holds after its proofs (its own high-water mark, keys and contexts aside); the card's power limit is read in
+the same call."""
 import json
 import os
 import sys
@@ -131,7 +138,142 @@ def measure_group(group, local, sizes, reps=None):
     return out if rank == 0 else None
 
 
+class _PeakMem:
+    """Samples the device's used memory every millisecond in a background thread (all parties share the device)."""
+
+    def __init__(self):
+        import threading
+        free, total = torch.cuda.mem_get_info(0)
+        self.base, self.peak, self.total, self.stop = total - free, 0, total, False
+        self.th = threading.Thread(target=self._run)
+        self.th.start()
+
+    def _run(self):
+        while not self.stop:
+            free, _ = torch.cuda.mem_get_info(0)
+            self.peak = max(self.peak, self.total - free - self.base)
+            time.sleep(0.001)
+
+    def done(self):
+        self.stop = True
+        self.th.join()
+        return self.peak
+
+
+def _party_threads(fn, n):
+    import threading
+    errs = []
+
+    def run(p):
+        try:
+            fn(p)
+        except Exception as e:  # noqa: BLE001
+            errs.append(e)
+    th = [threading.Thread(target=run, args=(p,)) for p in range(n)]
+    for t in th:
+        t.start()
+    for t in th:
+        t.join()
+    if errs:
+        raise errs[0]
+
+
+def measure_threads(sizes, num_parties, threshold, reps=None):
+    """Rep3 and Shamir(num_parties, threshold) co-Plonk, every party a thread on cuda:0 -> {"2p<lg>": {...}}."""
+    import random
+    from helpers import Conv, plonk_proof_from_device
+    from oracle import plonk as OP
+    from oracle.fields import BN254
+    from oracle.pairing_bn254 import pairing_product_is_one
+    reps = reps or int(os.environ.get("CS_CO_PLONK_REPS", "3"))
+    cv = Conv("bn254")
+    import subprocess
+    power = subprocess.run(["nvidia-smi", "-i", "0", "--query-gpu=power.limit", "--format=csv,noheader,nounits"],
+                           capture_output=True, text=True).stdout.strip()  # read-only query, part of the numbers
+    out = {"gpu": torch.cuda.get_device_name(0), "power_limit_w": power, "shamir": [num_parties, threshold]}
+    for lg in sizes:
+        ctx0 = B.Context(0)
+        t_setup = time.time()
+        syn = SynthPlonk(ctx0, lg)
+        setup_s = time.time() - t_setup
+        ctx0.close()
+        npub, wit = syn.n_public, syn.full_witness[syn.n_public + 1:]
+        rng = random.Random(lg)
+        row = {"setup_s": round(setup_s, 1)}
+        # ---- Rep3: three threads, products stored straight into the next party's arena (same-process pointers)
+        s0 = [rng.randrange(R) for _ in wit]
+        s1 = [rng.randrange(R) for _ in wit]
+        sh = [s0, s1, [(x - a - b) % R for x, a, b in zip(wit, s0, s1)]]
+        mine = [np.stack([cv.fr(sh[p]), cv.fr(sh[(p + 2) % 3])], axis=1) for p in range(3)]
+        ctxs = [B.Context(0) for _ in range(3)]
+        pks = [B.PlonkKey(c, B.CS_BN254, syn.key) for c in ctxs]
+        sess = [B.PlonkRep3Session(ctxs[p], pks[p], p) for p in range(3)]
+        nets = [B.Net.peer(ctxs[p], p, 3) for p in range(3)]
+        for x in nets:
+            x.connect_local(nets)
+        for p in range(3):
+            sess[p].connect(sess[(p + 1) % 3].arena)
+            sess[p].connect_io(sess[(p + 2) % 3].d_out, sess[(p + 1) % 3].d_out)
+        seeds = [bytes((31 * p + i) & 0xff for i in range(32)) for p in range(3)]
+        states = [B.Rep3StateC.from_seeds(ctxs[0].lib, p, seeds[p], seeds[(p + 2) % 3]) for p in range(3)]
+        ms, res = [], {}
+        for i in range(reps):
+            sent0 = [x.bytes_sent for x in nets]
+            t0 = time.perf_counter()
+            _party_threads(lambda p: res.__setitem__(p, sess[p].prove(nets[p], states[p], syn.public_inputs, mine[p])), 3)
+            ms.append((time.perf_counter() - t0) * 1e3)
+        proof = plonk_proof_from_device(cv, *res[0])
+        row["rep3"] = {"ms_per_proof": round(min(ms[1:] or ms), 1), "all_ms": [round(x, 1) for x in ms],
+                       "verified": bool(OP.verify(BN254, syn.vk_ints(), proof, syn.full_witness[1:npub + 1], pairing_product_is_one)),
+                       "bytes_sent_per_party": max(x.bytes_sent - s for x, s in zip(nets, sent0))}
+        for x in sess + pks + nets + states:
+            x.free()
+        for c in ctxs:
+            c.close()
+        # ---- Shamir(n, t): degree-t shares of the witness
+        n, t = num_parties, threshold
+        co = [[rng.randrange(R) for _ in wit] for _ in range(t)]
+        shares = []
+        for p in range(n):
+            x = p + 1
+            shares.append(cv.fr([(v + sum(c[j] * pow(x, k + 1, R) for k, c in enumerate(co))) % R for j, v in enumerate(wit)]))
+        ctxs = [B.Context(0) for _ in range(n)]
+        pks = [B.PlonkKey(c, B.CS_BN254, syn.key) for c in ctxs]
+        sess = [B.PlonkShamirSession(ctxs[p], pks[p], n, t, p) for p in range(n)]
+        nets = [B.Net.peer(ctxs[p], p, n) for p in range(n)]
+        for x in nets:
+            x.connect_local(nets)
+        ms, pair_ms, res, peak = [], [], {}, 0
+        for i in range(reps):
+            sent0 = [x.bytes_sent for x in nets]
+            mon = _PeakMem()
+            t0 = time.perf_counter()
+            _party_threads(lambda p: res.__setitem__(p, sess[p].prove(nets[p], syn.public_inputs, shares[p])), n)
+            ms.append((time.perf_counter() - t0) * 1e3)
+            peak = max(peak, mon.done())
+            pair_ms.append(max(s.pair_ms() for s in sess))
+        proof = plonk_proof_from_device(cv, *res[0][:2])
+        k = ms.index(min(ms[1:] or ms))
+        row["shamir"] = {"ms_per_proof": round(ms[k], 1), "pair_generation_ms": round(pair_ms[k], 1),
+                         "rounds_ms": round(ms[k] - pair_ms[k], 1), "all_ms": [round(x, 1) for x in ms],
+                         "verified": bool(OP.verify(BN254, syn.vk_ints(), proof, syn.full_witness[1:npub + 1], pairing_product_is_one)),
+                         "pairs": sess[0].pairs(), "pairs_formula_58n_13": 58 * syn.n + 13,
+                         "bytes_sent_per_party": [x.bytes_sent - s for x, s in zip(nets, sent0)],
+                         "peak_device_bytes_all_parties": int(peak),
+                         "session_device_bytes_per_party": [x.device_bytes() for x in sess]}
+        for x in sess + pks + nets:
+            x.free()
+        for c in ctxs:
+            c.close()
+        out["2p%d" % lg] = row
+        print(json.dumps({"2p%d" % lg: row}), file=sys.stderr, flush=True)
+    return out
+
+
 if __name__ == "__main__":
+    if len(sys.argv) > 3 and sys.argv[1] == "--shamir":
+        print(json.dumps(measure_threads([int(a) for a in sys.argv[4:]] or [20], int(sys.argv[2]), int(sys.argv[3]))))
+        sys.exit(0)
     res = measure([int(a) for a in sys.argv[1:]] or [16, 18])
     if res is not None:
         print(json.dumps(res))

@@ -110,8 +110,10 @@ int cs_ctx_create(int device, void* stream, cs_ctx** out) {
   CS_CUDA(cudaEventCreateWithFlags(&ctx->ev_wm, cudaEventDisableTiming));
   CS_CUDA(cudaEventCreateWithFlags(&ctx->ev_fork, cudaEventDisableTiming));
   CS_TRY(ntt_smem_optin<Bn254Fr>());
+  CS_TRY(msm_smem_optin<Bn254Fr>());
 #if defined(CS_ENABLE_BLS12_381)
   CS_TRY(ntt_smem_optin<Bls381Fr>());
+  CS_TRY(msm_smem_optin<Bls381Fr>());
 #endif
   *out = ctx;
   return 0;

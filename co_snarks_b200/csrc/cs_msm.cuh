@@ -25,21 +25,12 @@ constexpr unsigned MSM_ORDER_BLOCK = 256;
 constexpr unsigned MSM_RED_SEG = 4;     // buckets per thread in the weighted bucket reduction
 constexpr unsigned MSM_SIGN = 0x80000000u;
 
-// --------------------------------------------------------------------------- digits + histogram
-// One thread per scalar: optional Montgomery -> canonical, signed c-bit recoding, histogram.
-template <class FrP>
-CS_GLOBAL void k_msm_digits(const uint32_t* __restrict__ scalars, uint32_t sstride, uint32_t n, int mont,
-                            uint32_t c, uint32_t W, const uint32_t* __restrict__ infmask, uint32_t offset,
-                            uint32_t* __restrict__ dig, uint32_t* __restrict__ count) {
-  uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= n) return;
-  // bases at infinity (sparse Groth16 B-queries: B_i(tau) = 0 for variables absent from B) contribute
-  // nothing: drop their entries before the sort instead of carrying them through the accumulation.
-  // infmask = null: keep every entry (the witness sort that several base sets share, filtered per table by k_msm_view_*)
-  if (infmask && ((infmask[(offset + i) >> 5] >> ((offset + i) & 31)) & 1)) {
-    for (uint32_t w = 0; w < W; w++) dig[(size_t)w * n + i] = 0;
-    return;
-  }
+// --------------------------------------------------------------------------- digits
+// Scalar i: optional Montgomery -> canonical, then signed c-bit recoding; f(w, digit) for every window w, where the
+// digit is bucket | MSM_SIGN and bucket 0 is a zero digit.
+template <class FrP, class Fn>
+CS_D void msm_recode(const uint32_t* __restrict__ scalars, uint32_t sstride, uint32_t i, int mont, uint32_t c,
+                     uint32_t W, Fn&& f) {
   Fp<FrP> s;
   // sstride = elements between consecutive scalars (2 reads the `a` component of Rep3 shares in place)
   const uint4* src = reinterpret_cast<const uint4*>(scalars) + (size_t)i * sstride * (FrP::N / 4);
@@ -49,18 +40,14 @@ CS_GLOBAL void k_msm_digits(const uint32_t* __restrict__ scalars, uint32_t sstri
     s.l[4 * k] = v.x; s.l[4 * k + 1] = v.y; s.l[4 * k + 2] = v.z; s.l[4 * k + 3] = v.w;
   }
   if (mont) s = s.from_mont();
-  uint32_t lim[FrP::N + 1];
-  CS_UNROLL
-  for (int k = 0; k < FrP::N; k++) lim[k] = s.l[k];
-  lim[FrP::N] = 0;
   const uint32_t half = 1u << (c - 1);
   const uint32_t mask = (1u << c) - 1;
   uint32_t carry = 0;
   for (uint32_t w = 0; w < W; w++) {
     uint32_t pos = w * c;
     uint32_t li = pos >> 5, sh = pos & 31;
-    uint32_t lo = li < FrP::N ? lim[li] : 0;
-    uint32_t hi = li + 1 < FrP::N ? lim[li + 1] : 0;
+    uint32_t lo = li < FrP::N ? s.l[li] : 0;
+    uint32_t hi = li + 1 < FrP::N ? s.l[li + 1] : 0;
     uint32_t d = (__funnelshift_r(lo, hi, sh) & mask) + carry;
     uint32_t out;
     if (d > half) {
@@ -70,9 +57,106 @@ CS_GLOBAL void k_msm_digits(const uint32_t* __restrict__ scalars, uint32_t sstri
       out = d;
       carry = 0;
     }
-    dig[(size_t)w * n + i] = out;
-    uint32_t b = out & ~MSM_SIGN;
-    if (b) atomicAdd(&count[b], 1u);
+    f(w, out);
+  }
+}
+
+// bases at infinity (sparse Groth16 B-queries: B_i(tau) = 0 for variables absent from B) contribute nothing: their
+// entries are dropped before the sort instead of being carried through the accumulation.  infmask = null keeps every
+// entry (the witness sort that several base sets share, filtered per table by k_msm_view_*).
+CS_D bool msm_base_inf(const uint32_t* __restrict__ infmask, uint32_t k) {
+  return infmask && ((infmask[k >> 5] >> (k & 31)) & 1);
+}
+
+// --------------------------------------------------------------------------- bucket sort
+// A counting sort of the W n entries by bucket in three passes, with no global atomics:
+//  * k_msm_bin_count: block x takes scalars [x tile, (x + 1) tile), recodes them and counts its entries per bucket in a
+//    shared-memory histogram; the histogram becomes row x of tab (nblk rows of B words, column b - 1 = bucket b).
+//  * k_msm_bin_scan: per bucket, the rows become exclusive prefixes (block x's first slot inside the bucket) and the
+//    column total becomes count[b].
+//  * k_msm_bin_scatter: the block recodes its tile again and places every entry at start[b] + its row's prefix + a
+//    rank from a shared-memory cursor.
+// A histogram covers MSM_BIN_SPAN buckets (128 KB); wider windows split the buckets over grid.y, and each block
+// re-reads its tile for its share of the buckets.  The scatter takes MSM_SCATTER_SPAN buckets per grid.y slice even
+// at c = 16: its scattered 4-byte stores, not the recoding, bound it, and with a quarter of the buckets at a time the
+// output lines being written stay fewer (measured at 2^20 scalars on the H100: 412 us in four slices against 509 us
+// in one, although each slice recodes the tile again).
+constexpr unsigned MSM_BIN_T = 1024;             // threads per block of k_msm_bin_count / k_msm_bin_scatter
+constexpr unsigned MSM_BIN_TILE = 4096;          // scalars per block, unless the count table would outgrow W n words
+constexpr unsigned MSM_BIN_SPAN = 1u << 15;      // buckets per shared-memory histogram: all of them up to c = 16
+constexpr unsigned MSM_SCATTER_SPAN = 1u << 13;  // buckets per grid.y slice of k_msm_bin_scatter
+
+template <class FrP>
+CS_GLOBAL void __launch_bounds__(MSM_BIN_T) k_msm_bin_count(const uint32_t* __restrict__ scalars, uint32_t sstride,
+                                                            uint32_t n, int mont, uint32_t c, uint32_t W,
+                                                            const uint32_t* __restrict__ infmask, uint32_t offset,
+                                                            uint32_t tile, uint32_t B, uint32_t* __restrict__ tab) {
+  CS_DYN_SMEM(uint32_t, h);
+  const uint32_t lo = blockIdx.y * MSM_BIN_SPAN + 1;  // buckets [lo, lo + span)
+  const uint32_t span = B + 1 - lo < MSM_BIN_SPAN ? B + 1 - lo : MSM_BIN_SPAN;
+  for (uint32_t k = threadIdx.x; k < span; k += blockDim.x) h[k] = 0;
+  __syncthreads();
+  const uint32_t i1 = (blockIdx.x + 1) * tile < n ? (blockIdx.x + 1) * tile : n;
+  for (uint32_t i = blockIdx.x * tile + threadIdx.x; i < i1; i += blockDim.x) {
+    if (msm_base_inf(infmask, offset + i)) continue;
+    msm_recode<FrP>(scalars, sstride, i, mont, c, W, [&](uint32_t, uint32_t d) {
+      const uint32_t k = (d & ~MSM_SIGN) - lo;  // wraps past span for bucket 0 and for buckets below lo
+      if (k < span) atomicAdd(&h[k], 1u);
+    });
+  }
+  __syncthreads();
+  uint32_t* row = tab + (size_t)blockIdx.x * B + (lo - 1);
+  for (uint32_t k = threadIdx.x; k < span; k += blockDim.x) row[k] = h[k];
+}
+
+// One thread per bucket, down the nblk rows of its column; count[0] = 0 (zero digits are dropped).
+constexpr unsigned MSM_BIN_SCAN_U = 16;  // rows loaded before any is rewritten: loads in flight per thread
+static CS_GLOBAL void k_msm_bin_scan(uint32_t* __restrict__ tab, uint32_t nblk, uint32_t B, uint32_t* __restrict__ count) {
+  const uint32_t b = blockIdx.x * blockDim.x + threadIdx.x;
+  if (b == 0) count[0] = 0;
+  if (b >= B) return;
+  uint32_t* col = tab + b;
+  uint32_t run = 0, r = 0;
+  for (; r + MSM_BIN_SCAN_U <= nblk; r += MSM_BIN_SCAN_U) {
+    uint32_t v[MSM_BIN_SCAN_U];
+    CS_UNROLL
+    for (uint32_t u = 0; u < MSM_BIN_SCAN_U; u++) v[u] = col[(size_t)(r + u) * B];
+    CS_UNROLL
+    for (uint32_t u = 0; u < MSM_BIN_SCAN_U; u++) {
+      col[(size_t)(r + u) * B] = run;
+      run += v[u];
+    }
+  }
+  for (; r < nblk; r++) {
+    const uint32_t v = col[(size_t)r * B];
+    col[(size_t)r * B] = run;
+    run += v;
+  }
+  count[b + 1] = run;
+}
+
+// sorted[pos] = table slot w * nbases + offset + i | sign, grouped by bucket
+template <class FrP>
+CS_GLOBAL void __launch_bounds__(MSM_BIN_T) k_msm_bin_scatter(const uint32_t* __restrict__ scalars, uint32_t sstride,
+                                                              uint32_t n, int mont, uint32_t c, uint32_t W,
+                                                              const uint32_t* __restrict__ infmask, uint32_t offset,
+                                                              uint32_t tile, uint32_t B, uint32_t nbases,
+                                                              const uint32_t* __restrict__ tab,
+                                                              const uint32_t* __restrict__ start,
+                                                              uint32_t* __restrict__ sorted) {
+  CS_DYN_SMEM(uint32_t, cur);
+  const uint32_t lo = blockIdx.y * MSM_SCATTER_SPAN + 1;
+  const uint32_t span = B + 1 - lo < MSM_SCATTER_SPAN ? B + 1 - lo : MSM_SCATTER_SPAN;
+  const uint32_t* row = tab + (size_t)blockIdx.x * B + (lo - 1);
+  for (uint32_t k = threadIdx.x; k < span; k += blockDim.x) cur[k] = start[lo + k] + row[k];
+  __syncthreads();
+  const uint32_t i1 = (blockIdx.x + 1) * tile < n ? (blockIdx.x + 1) * tile : n;
+  for (uint32_t i = blockIdx.x * tile + threadIdx.x; i < i1; i += blockDim.x) {
+    if (msm_base_inf(infmask, offset + i)) continue;
+    msm_recode<FrP>(scalars, sstride, i, mont, c, W, [&](uint32_t w, uint32_t d) {
+      const uint32_t k = (d & ~MSM_SIGN) - lo;
+      if (k < span) sorted[atomicAdd(&cur[k], 1u)] = (w * nbases + offset + i) | (d & MSM_SIGN);
+    });
   }
 }
 
@@ -169,24 +253,9 @@ static CS_GLOBAL void k_msm_scan2(const uint32_t* __restrict__ count, uint32_t n
   }
 }
 
-// --------------------------------------------------------------------------- scatter
-// grid.y = window.  sorted[pos] = table index | sign, grouped by bucket.
-static CS_GLOBAL void k_msm_scatter(const uint32_t* __restrict__ dig, uint32_t n, uint32_t nbases,
-                             uint32_t offset, const uint32_t* __restrict__ start,
-                             uint32_t* __restrict__ cursor, uint32_t* __restrict__ sorted) {
-  uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
-  uint32_t w = blockIdx.y;
-  if (i >= n) return;
-  uint32_t d = dig[(size_t)w * n + i];
-  uint32_t b = d & ~MSM_SIGN;
-  if (!b) return;
-  uint32_t pos = start[b] + atomicAdd(&cursor[b], 1u);
-  sorted[pos] = (w * nbases + offset + i) | (d & MSM_SIGN);
-}
-
 // --------------------------------------------------------------------------- filtered view of a shared sort
 // Groth16's A, B1, B2 and L MSMs take the same witness scalars over different tables.  Their digits are sorted ONCE
-// without an infinity mask (k_msm_digits with infmask = null, entries w * n + i: window w, scalar i); a table with
+// without an infinity mask (msm_sort with infmask = null, entries w * n + i: window w, scalar i); a table with
 // infinity bases, or whose slots are not w * n + i, gets a stream compaction of those entries that drops the entries
 // of its infinite bases and rewrites the rest to its own slots, w * nbases + offset + i.  The compaction keeps the
 // order, so the view is grouped by bucket as the shared entries are, and its bucket counts follow from the kept
@@ -709,20 +778,19 @@ struct MsmSizes {
     max_s2 = max_s1 / S + nb1;
     ob = ceil_div(max_s0, MSM_ORDER_BLOCK);
   }
-  // meta: count[nb1] cursor[nb1] | start[nb1+1] sstart0[nb1+1] sstart1[nb1+1] sstart2[nb1+1] | aux[4 * scan blocks]
-  size_t meta_words() const { return 2 * (size_t)nb1 + 4 * ((size_t)nb1 + 1) + 4 * MSM_SCAN_MAX_BLOCKS; }
+  // meta: count[nb1] | start[nb1+1] sstart0[nb1+1] sstart1[nb1+1] sstart2[nb1+1] | aux[4 * scan blocks]
+  size_t meta_words() const { return (size_t)nb1 + 4 * ((size_t)nb1 + 1) + 4 * MSM_SCAN_MAX_BLOCKS; }
   // slice order: slice_len | slice_bkt | order | order_b (max_s0 each) | block_hist | len_base | chunk_sum
   size_t order_words() const {
     return 4 * max_s0 + (size_t)ob * (MSM_SLICE_MAX + 1) + 2 * (MSM_SLICE_MAX + 1) + (size_t)(MSM_SLICE_MAX + 1) * MSM_OFF_CHUNKS;
   }
 };
 struct MsmSortBufs {
-  uint32_t *count, *cursor, *start, *sstart0, *sstart1, *sstart2, *aux;
+  uint32_t *count, *start, *sstart0, *sstart1, *sstart2, *aux;
   uint32_t *slice_len, *slice_bkt, *order, *order_b, *block_hist, *len_base, *chunk_sum;
   MsmSortBufs(const MsmWorkspace& w, const MsmSizes& z) {
     count = w.meta.as<uint32_t>();
-    cursor = count + z.nb1;
-    start = cursor + z.nb1;
+    start = count + z.nb1;
     sstart0 = start + z.nb1 + 1;
     sstart1 = sstart0 + z.nb1 + 1;
     sstart2 = sstart1 + z.nb1 + 1;
@@ -772,6 +840,24 @@ static inline int msm_slice_order(MsmWorkspace& ws, const MsmSortBufs& q, const 
   return 0;
 }
 
+// The bucket sort's histograms take more than the default 48 KB of shared memory; once per device and scalar field.
+template <class FrP>
+int msm_smem_optin() {
+#if !defined(CS_EMU)
+  CS_CUDA(cudaFuncSetAttribute(k_msm_bin_count<FrP>, cudaFuncAttributeMaxDynamicSharedMemorySize, MSM_BIN_SPAN * 4));
+  CS_CUDA(cudaFuncSetAttribute(k_msm_bin_scatter<FrP>, cudaFuncAttributeMaxDynamicSharedMemorySize, MSM_SCATTER_SPAN * 4));
+#endif
+  return 0;
+}
+
+// Scalars per block of the bucket sort: MSM_BIN_TILE, or more where nblk rows of B counts would exceed the W n words
+// the table has (windows above 16 at small n).  The table then takes at most max(W n, B) words.
+static inline uint32_t msm_bin_tile(const MsmShape& sh, const MsmSizes& z, uint32_t n) {
+  const size_t rows = z.nent / sh.B > 1 ? z.nent / sh.B : 1;
+  const size_t nblk = ceil_div(n, MSM_BIN_TILE) < rows ? ceil_div(n, MSM_BIN_TILE) : rows;
+  return n ? ceil_div(n, nblk) : 1;
+}
+
 // Digits, bucket sort and slice order of n scalars into ws; the entries index table slots w * nbases + offset + i.
 // infmask = null keeps the entries of every base: with nbases = n and offset = 0 that is the shared witness sort,
 // which msm_enqueue reads as it is (a table without infinity bases and slots w * n + i) or through msm_view.
@@ -780,19 +866,29 @@ int msm_sort(MsmWorkspace& ws, const uint32_t* infmask, uint32_t nbases, MsmShap
              const uint32_t* d_scalars, uint32_t sstride, uint32_t n, int mont, cudaStream_t st) {
   CS_TRY(msm_check_limits(sh, n, nbases));
   const MsmSizes z(sh, n);
-  CS_TRY(ws.dig.reserve(z.nent * 4));
+  const uint32_t tile = msm_bin_tile(sh, z, n);
+  const uint32_t nblk = n ? ceil_div(n, tile) : 0;
+  const dim3 grid(nblk, ceil_div(sh.B, MSM_BIN_SPAN)), grid_sc(nblk, ceil_div(sh.B, MSM_SCATTER_SPAN));
+  const uint32_t smem = (sh.B < MSM_BIN_SPAN ? sh.B : MSM_BIN_SPAN) * 4;
+  const uint32_t smem_sc = (sh.B < MSM_SCATTER_SPAN ? sh.B : MSM_SCATTER_SPAN) * 4;
+  // dig holds the per-block count table (k_msm_bin_*)
+  const size_t tab_words = (size_t)nblk * sh.B;
+  CS_TRY(ws.dig.reserve((tab_words > z.nent ? tab_words : z.nent) * 4));
   CS_TRY(ws.sorted.reserve(z.nent * 4));
   CS_TRY(ws.meta.reserve(z.meta_words() * 4));
   CS_TRY(ws.order.reserve(z.order_words() * 4));
   const MsmSortBufs q(ws, z);
+  uint32_t* tab = ws.dig.as<uint32_t>();
   CS_TRY(ws.mark(0, st));
-  CS_CUDA(cudaMemsetAsync(q.count, 0, 2 * (size_t)z.nb1 * 4, st));
-  CS_LAUNCH(k_msm_digits<FrP>, ceil_div(n, 256), 256, 0, st, d_scalars, sstride, n, mont, sh.c, sh.W, infmask, offset,
-            ws.dig.as<uint32_t>(), q.count);
+  if (nblk)
+    CS_LAUNCH_SYNC(k_msm_bin_count<FrP>, grid, MSM_BIN_T, smem, st, d_scalars, sstride, n, mont, sh.c, sh.W, infmask,
+                   offset, tile, sh.B, tab);
   CS_TRY(ws.mark(1, st));
+  CS_LAUNCH(k_msm_bin_scan, ceil_div(sh.B, 256), 256, 0, st, tab, nblk, sh.B, q.count);
   CS_TRY(msm_scan(q, z, sh.B, st));
-  CS_LAUNCH(k_msm_scatter, dim3(ceil_div(n, 256), sh.W), 256, 0, st, ws.dig.as<uint32_t>(), n, nbases, offset, q.start,
-            q.cursor, ws.sorted.as<uint32_t>());
+  if (nblk)
+    CS_LAUNCH_SYNC(k_msm_bin_scatter<FrP>, grid_sc, MSM_BIN_T, smem_sc, st, d_scalars, sstride, n, mont, sh.c, sh.W, infmask,
+                   offset, tile, sh.B, nbases, tab, q.start, ws.sorted.as<uint32_t>());
   return msm_slice_order(ws, q, z, st);
 }
 

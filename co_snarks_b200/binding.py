@@ -139,6 +139,9 @@ SIGNATURES = {
     "cs_bases_upload": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_size_t, C.c_int, C.POINTER(C.c_void_p)]),
     "cs_bases_free": (None, [C.c_void_p]),
     "cs_bases_len": (C.c_size_t, [C.c_void_p]),
+    "cs_bases_info": (C.c_int, [C.c_void_p, C.POINTER(C.c_uint), C.POINTER(C.c_uint), C.POINTER(C.c_uint), C.POINTER(C.c_size_t)]),
+    "cs_ctx_set_table_budget": (C.c_int, [C.c_void_p, C.c_size_t]),
+    "cs_groth16_pk_table_info": (C.c_int, [C.c_void_p, C.POINTER(C.c_uint), C.POINTER(C.c_size_t)]),
     "cs_msm": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_int, C.c_void_p, C.POINTER(C.c_int)]),
     "cs_msm_device": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_int, C.c_void_p, C.POINTER(C.c_int)]),
     "cs_msm_rep3_shares": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p]),
@@ -323,6 +326,10 @@ class Context:
 
     def launch_count(self):
         return int(self.lib.cs_ctx_launch_count(self.h))
+
+    def set_table_budget(self, nbytes):
+        """Cap the device bytes of base sets and keys created from now on (cs_ctx_set_table_budget); 0 = automatic."""
+        self._check(self.lib.cs_ctx_set_table_budget(self.h, int(nbytes)))
 
     # ---- device memory
     def alloc(self, nbytes):
@@ -513,6 +520,12 @@ class Bases:
 
     def __len__(self):
         return int(self.ctx.lib.cs_bases_len(self.h))
+
+    def info(self):
+        """-> dict(window_bits, windows, table_rows, device_bytes) (cs_bases_info)"""
+        c, w, t, nb = C.c_uint(), C.c_uint(), C.c_uint(), C.c_size_t()
+        self.ctx._check(self.ctx.lib.cs_bases_info(self.h, C.byref(c), C.byref(w), C.byref(t), C.byref(nb)))
+        return {"window_bits": c.value, "windows": w.value, "table_rows": t.value, "device_bytes": nb.value}
 
     def free(self):
         if self.h:
@@ -804,6 +817,12 @@ class Groth16Key:
         self.nw = d.num_witness_variables
         self.fq = limbs_of(curve, "fq")
         del keep
+
+    def table_info(self):
+        """-> (table rows, table device bytes) of the key's MSM tables (cs_groth16_pk_table_info)"""
+        rows, nb = C.c_uint(), C.c_size_t()
+        self.ctx._check(self.ctx.lib.cs_groth16_pk_table_info(self.h, C.byref(rows), C.byref(nb)))
+        return rows.value, nb.value
 
     @classmethod
     def from_zkey(cls, ctx, path, curve=None, window_bits=0):

@@ -188,28 +188,59 @@ int cs_memcpy_d2h(cs_ctx* ctx, void* h_dst, const void* d_src, size_t bytes) {
 // ------------------------------------------------------------------------------------------- MSM
 namespace cs {
 
-// widest window an MSM can run: msm_scan takes 2^20 bucket slots, 2^(c-1) buckets plus bucket 0
-constexpr unsigned MSM_MAX_WINDOW = 20;
-static_assert((1u << (MSM_MAX_WINDOW - 1)) + 1 <= MSM_SCAN_MAX_BLOCKS * MSM_SCAN_T, "MSM_MAX_WINDOW exceeds the scan");
+int table_budget(cs_ctx* ctx, size_t* out) {
+  size_t avail = 0, total = 0;
+#if defined(CS_EMU)
+  avail = total = 80ull << 30;  // the CPU emulation has no device: an 80 GB H100's, so full tables are picked as there
+#else
+  CS_CUDA(cudaMemGetInfo(&avail, &total));
+#endif
+  avail = avail > TABLE_MARGIN ? avail - TABLE_MARGIN : 0;
+  *out = ctx->table_budget && ctx->table_budget < avail ? ctx->table_budget : avail;
+  return 0;
+}
+
+int pick_table_rows(cs_ctx* ctx, unsigned c, unsigned W, const std::function<size_t(unsigned)>& need, const char* who,
+                    unsigned* k_out) {
+  size_t budget = 0, least = SIZE_MAX;
+  CS_TRY(table_budget(ctx, &budget));
+  for (unsigned k = 1; k <= W; k++) {
+    if ((size_t)k * (1u << (c - 1)) + 1 > (size_t)MSM_SCAN_MAX_BLOCKS * MSM_SCAN_T) break;  // k B buckets: msm_scan's limit
+    const size_t b = need(k);  // not monotone in k: k B buckets of scratch can outweigh the rows saved on tiny tables
+    if (b <= budget) {
+      *k_out = k;
+      return 0;
+    }
+    least = b < least ? b : least;
+  }
+  return fail(CS_ERR_LIMIT, "%s: the MSM tables need at least %zu bytes of device memory, %zu are available", who, least,
+              budget);
+}
 
 template <class Cfg, int G>
-int bases_upload_t(cs_ctx* ctx, const uint64_t* h_points, size_t n, int window_bits, cs_bases* b) {
+int bases_upload_t(cs_ctx* ctx, const uint64_t* h_points, size_t n, int window_bits, unsigned k, cs_bases* b) {
   typedef typename GroupOf<Cfg, G>::F F;
   unsigned c = window_bits ? (unsigned)window_bits : msm_auto_window(n, Cfg::FR_BITS);
   // a window wider than msm_scan takes would build the table and then fail every MSM
   if (c < 2 || c > MSM_MAX_WINDOW)
     return fail(CS_ERR_ARG, "cs_bases_upload: window_bits %d out of range [2,%u] (0 = automatic)", window_bits, MSM_MAX_WINDOW);
-  b->sh = msm_shape(Cfg::FR_BITS, c);
+  if (!k) {
+    const unsigned W = msm_shape(Cfg::FR_BITS, c).W;
+    CS_TRY(pick_table_rows(ctx, c, W, [&](unsigned kk) { return bases_bytes<Cfg, G>(n, msm_shape(Cfg::FR_BITS, c, kk)); },
+                           "cs_bases_upload", &k));
+  }
+  b->sh = msm_shape(Cfg::FR_BITS, c, k);
   b->n = n;
-  size_t total = (size_t)b->sh.W * n;
-  if (total >= (1ull << 31)) return fail(CS_ERR_LIMIT, "cs_bases_upload: W*n = %zu exceeds 2^31", total);
+  size_t total = (size_t)b->sh.T * n;
+  if (total >= (1ull << 31)) return fail(CS_ERR_LIMIT, "cs_bases_upload: T*n = %zu table slots exceed 2^31", total);
   CS_TRY(b->table.reserve(total * sizeof(Affine<F>)));
   CS_CUDA(cudaMemcpyAsync(b->table.p, h_points, n * sizeof(Affine<F>), cudaMemcpyHostToDevice, ctx->stream));
   CS_TRY(b->infmask.reserve(((n + 31) / 32) * 4));
   CS_LAUNCH(k_msm_infmask<F>, ceil_div((n + 31) / 32, 128), 128, 0, ctx->stream, b->table.as<Affine<F>>(), (uint32_t)n,
             b->infmask.as<uint32_t>());
+  // row j = 2^(c k j) P_i: the full-table precomputation with a window of c k bits
   CS_LAUNCH(k_msm_precompute<F>, ceil_div(n, 128), 128, 0, ctx->stream, b->table.as<Affine<F>>(), (uint32_t)n,
-            b->sh.c, b->sh.W);
+            b->sh.c * b->sh.k, b->sh.T);
   // BN254 G1, opt-in (CS_MSM_F52=1): bucket accumulation on the FP64 pipe (cs_msm52.cuh); its table holds the
   // coordinates in the radix-2^260 Montgomery form.  Bit-exact, but the FP64 and integer pipes do not overlap, so
   // trading IMAD.WIDE for DFMA buys nothing: the integer kernel stays the default.
@@ -264,6 +295,23 @@ int msm_sort_shared_dyn(cs_ctx* ctx, int slot, cudaStream_t st, const cs_bases* 
   return 0;
 }
 
+int bases_upload(cs_ctx* ctx, cs_curve curve, cs_group group, const uint64_t* h_points_mont, size_t n, int window_bits,
+                 unsigned k, cs_bases** out) {
+  if (!ctx || !h_points_mont || !out) return fail(CS_ERR_ARG, "cs_bases_upload: NULL argument");
+  if (n == 0) return fail(CS_ERR_ARG, "cs_bases_upload: empty base set");
+  if (group != CS_G1 && group != CS_G2) return fail(CS_ERR_ARG, "cs_bases_upload: bad group %d", (int)group);
+  CS_CUDA(cudaSetDevice(ctx->device));
+  std::unique_ptr<cs_bases, void (*)(cs_bases*)> b(new cs_bases(), cs_bases_free);  // a failed upload frees its buffers
+  b->curve = curve;
+  b->group = group;
+  CS_DISPATCH_CURVE(curve, {
+    if (group == CS_G1) CS_TRY((bases_upload_t<Cfg, 0>(ctx, h_points_mont, n, window_bits, k, b.get())));
+    else CS_TRY((bases_upload_t<Cfg, 1>(ctx, h_points_mont, n, window_bits, k, b.get())));
+  });
+  *out = b.release();
+  return 0;
+}
+
 int msm_finish_dyn(cs_ctx* ctx, int slot, const cs_bases* b, uint64_t* out_affine, int* out_inf) {
   CS_DISPATCH_CURVE(b->curve, {
     if (b->group == CS_G1) msm_finish_t<Cfg, 0>(ctx, slot, out_affine, out_inf);
@@ -276,21 +324,15 @@ int msm_finish_dyn(cs_ctx* ctx, int slot, const cs_bases* b, uint64_t* out_affin
 
 extern "C" {
 
+int cs_ctx_set_table_budget(cs_ctx* ctx, size_t bytes) {
+  if (!ctx) return fail(CS_ERR_ARG, "ctx is NULL");
+  ctx->table_budget = bytes;
+  return 0;
+}
+
 int cs_bases_upload(cs_ctx* ctx, cs_curve curve, cs_group group, const uint64_t* h_points_mont, size_t n,
                     int window_bits, cs_bases** out) {
-  if (!ctx || !h_points_mont || !out) return fail(CS_ERR_ARG, "cs_bases_upload: NULL argument");
-  if (n == 0) return fail(CS_ERR_ARG, "cs_bases_upload: empty base set");
-  if (group != CS_G1 && group != CS_G2) return fail(CS_ERR_ARG, "cs_bases_upload: bad group %d", (int)group);
-  CS_CUDA(cudaSetDevice(ctx->device));
-  std::unique_ptr<cs_bases> b(new cs_bases());
-  b->curve = curve;
-  b->group = group;
-  CS_DISPATCH_CURVE(curve, {
-    if (group == CS_G1) CS_TRY((bases_upload_t<Cfg, 0>(ctx, h_points_mont, n, window_bits, b.get())));
-    else CS_TRY((bases_upload_t<Cfg, 1>(ctx, h_points_mont, n, window_bits, b.get())));
-  });
-  *out = b.release();
-  return 0;
+  return bases_upload(ctx, curve, group, h_points_mont, n, window_bits, 0, out);
 }
 
 void cs_bases_free(cs_bases* b) {
@@ -301,6 +343,15 @@ void cs_bases_free(cs_bases* b) {
 }
 
 size_t cs_bases_len(const cs_bases* b) { return b ? b->n : 0; }
+
+int cs_bases_info(const cs_bases* b, unsigned* window_bits, unsigned* windows, unsigned* table_rows, size_t* device_bytes) {
+  if (!b) return fail(CS_ERR_ARG, "cs_bases_info: bases is NULL");
+  if (window_bits) *window_bits = b->sh.c;
+  if (windows) *windows = b->sh.W;
+  if (table_rows) *table_rows = b->sh.T;
+  if (device_bytes) *device_bytes = b->table.cap + b->infmask.cap;
+  return 0;
+}
 
 int cs_msm_device(cs_ctx* ctx, const cs_bases* b, size_t offset, const uint64_t* d_scalars, size_t n,
                   int scalars_montgomery, uint64_t* h_out, int* out_inf) {

@@ -71,12 +71,14 @@ static inline unsigned ceil_div(size_t a, size_t b) { return (unsigned)((a + b -
 struct DevBuf {
   void* p = nullptr;
   size_t cap = 0;
+  // bytes reserve(bytes) allocates when the buffer has to grow
+  static size_t alloc_size(size_t bytes) { return bytes + (bytes >> 3) + 256; }
   int reserve(size_t bytes) {
     if (bytes <= cap) return 0;
     if (p) cudaFree(p);
     p = nullptr;
     cap = 0;
-    size_t want = bytes + (bytes >> 3) + 256;
+    size_t want = alloc_size(bytes);
     CS_CUDA(cudaMalloc(&p, want));
     cap = want;
     return 0;

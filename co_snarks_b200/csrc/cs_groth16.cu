@@ -255,7 +255,7 @@ int plan_witness_views(cs_ctx* ctx, cs_groth16_pk* pk) {
   const size_t off[4] = {ni, ni, ni, 0};
   std::vector<uint8_t> inf[4];
   for (int j = 0; j < 4; j++) {
-    if (q[j]->sh.c != q[0]->sh.c || q[j]->sh.W != q[0]->sh.W)
+    if (q[j]->sh.c != q[0]->sh.c || q[j]->sh.W != q[0]->sh.W || q[j]->sh.k != q[0]->sh.k)
       return fail(CS_ERR_STATE, "cs_groth16_pk_create: the witness MSMs' tables differ in window shape");
     std::vector<uint32_t> words((q[j]->n + 31) / 32);
     CS_CUDA(cudaMemcpyAsync(words.data(), q[j]->infmask.p, words.size() * 4, cudaMemcpyDeviceToHost, ctx->stream));
@@ -279,6 +279,27 @@ int plan_witness_views(cs_ctx* ctx, cs_groth16_pk* pk) {
       }
   }
   return 0;
+}
+
+// Device bytes of a key whose tables keep one row per k windows: its five tables, and what its proofs reserve, sized by
+// the code that reserves it -- the five MSM workspaces and the shared witness sort (msm_sort_bytes, msm_accum_bytes),
+// the witness-map vectors of a Rep3 proof (the larger share kind: two components, two masks), the coset table and
+// the domain's twiddles.  cw / ch: windows of the witness tables and of H.
+template <class Cfg>
+size_t key_bytes(size_t ni, size_t nw, size_t n, unsigned cw, unsigned ch, unsigned k) {
+  typedef typename GroupOf<Cfg, 0>::F F1;
+  typedef typename GroupOf<Cfg, 1>::F F2;
+  const MsmShape sw = msm_shape(Cfg::FR_BITS, cw, k), shh = msm_shape(Cfg::FR_BITS, ch, k);
+  size_t b = 2 * bases_bytes<Cfg, 0>(ni + nw, sw) + bases_bytes<Cfg, 1>(ni + nw, sw) + bases_bytes<Cfg, 0>(n, shh);
+  if (nw) {
+    b += bases_bytes<Cfg, 0>(nw, sw);
+    b += 5 * msm_sort_bytes(sw, (uint32_t)nw) + 3 * msm_accum_bytes<F1>(sw, (uint32_t)nw) + msm_accum_bytes<F2>(sw, (uint32_t)nw);
+  }
+  b += msm_sort_bytes(shh, (uint32_t)n) + msm_accum_bytes<F1>(shh, (uint32_t)n);
+  const size_t fr = 32;
+  b += DevBuf::alloc_size(ni * fr) + DevBuf::alloc_size(nw * 2 * fr) + 2 * DevBuf::alloc_size(n * 2 * fr) +
+       4 * DevBuf::alloc_size(n * fr) + 2 * DevBuf::alloc_size(n / 2 * fr);
+  return b;
 }
 
 int upload_inputs(cs_ctx* ctx, cs_groth16_pk* pk, int kind, const uint64_t* h_pub, const uint64_t* h_wit,
@@ -677,6 +698,12 @@ int cs_groth16_rep3_prove_helper(cs_ctx* ctx, cs_groth16_pk* pk, int party, cs_n
 }
 
 int cs_groth16_pk_create(cs_ctx* ctx, const cs_groth16_key_desc* d, cs_groth16_pk** out) {
+  return cs::groth16_pk_create(ctx, d, 0, out);
+}
+
+}  // extern "C"
+
+int cs::groth16_pk_create(cs_ctx* ctx, const cs_groth16_key_desc* d, unsigned k, cs_groth16_pk** out) {
   if (!ctx || !d || !out) return fail(CS_ERR_ARG, "cs_groth16_pk_create: NULL argument");
   if (d->curve != CS_BN254
 #if defined(CS_ENABLE_BLS12_381)
@@ -690,8 +717,10 @@ int cs_groth16_pk_create(cs_ctx* ctx, const cs_groth16_key_desc* d, cs_groth16_p
   if (d->a_query_len != ni + nw || d->b_g1_query_len != ni + nw || d->b_g2_query_len != ni + nw)
     return fail(CS_ERR_ARG, "cs_groth16_pk_create: a/b query length must be %zu", ni + nw);
   if (d->l_query_len != nw) return fail(CS_ERR_ARG, "cs_groth16_pk_create: l_query length must be %zu", nw);
+  if (d->window_bits && (d->window_bits < 2 || d->window_bits > (int)MSM_MAX_WINDOW))
+    return fail(CS_ERR_ARG, "cs_bases_upload: window_bits %d out of range [2,%u] (0 = automatic)", d->window_bits, MSM_MAX_WINDOW);
   CS_CUDA(cudaSetDevice(ctx->device));
-  std::unique_ptr<cs_groth16_pk> pk(new cs_groth16_pk());
+  std::unique_ptr<cs_groth16_pk, void (*)(cs_groth16_pk*)> pk(new cs_groth16_pk(), cs_groth16_pk_free);
   pk->curve = d->curve;
   pk->nc = nc; pk->ni = ni; pk->nw = nw;
   size_t n = 1;
@@ -728,13 +757,22 @@ int cs_groth16_pk_create(cs_ctx* ctx, const cs_groth16_key_desc* d, cs_groth16_p
   const int wb = d->window_bits;
   // A, B1, B2 and L share one sort of the witness digits, so their tables share one window shape: the one the
   // nw witness scalars would get (the MSMs run over nw scalars; the result does not depend on the window)
-  int wwb = wb;
-  if (!wwb) CS_DISPATCH_CURVE(d->curve, { wwb = (int)msm_auto_window(nw, Cfg::FR_BITS); });
-  CS_TRY(cs_bases_upload(ctx, d->curve, CS_G1, d->a_query, d->a_query_len, wwb, &pk->a_query));
-  CS_TRY(cs_bases_upload(ctx, d->curve, CS_G1, d->b_g1_query, d->b_g1_query_len, wwb, &pk->b_g1));
-  CS_TRY(cs_bases_upload(ctx, d->curve, CS_G2, d->b_g2_query, d->b_g2_query_len, wwb, &pk->b_g2));
-  if (nw) CS_TRY(cs_bases_upload(ctx, d->curve, CS_G1, d->l_query, d->l_query_len, wwb, &pk->l_query));
-  CS_TRY(cs_bases_upload(ctx, d->curve, CS_G1, d->h_query, n, wb, &pk->h_query));
+  int wwb = wb, hwb = wb;
+  // one k (windows per table row) for the five tables: the smallest with which the key fits the table budget
+  CS_DISPATCH_CURVE(d->curve, {
+    if (!wwb) wwb = (int)msm_auto_window(nw, Cfg::FR_BITS);
+    if (!hwb) hwb = (int)msm_auto_window(n, Cfg::FR_BITS);
+    const unsigned cmax = wwb > hwb ? wwb : hwb;
+    const unsigned W = msm_shape(Cfg::FR_BITS, wwb < hwb ? wwb : hwb).W;  // the more windows of the two shapes
+    if (!k)
+      CS_TRY(pick_table_rows(ctx, cmax, W, [&](unsigned kk) { return key_bytes<Cfg>(ni, nw, n, wwb, hwb, kk); },
+                             "cs_groth16_pk_create", &k));
+  });
+  CS_TRY(bases_upload(ctx, d->curve, CS_G1, d->a_query, d->a_query_len, wwb, k, &pk->a_query));
+  CS_TRY(bases_upload(ctx, d->curve, CS_G1, d->b_g1_query, d->b_g1_query_len, wwb, k, &pk->b_g1));
+  CS_TRY(bases_upload(ctx, d->curve, CS_G2, d->b_g2_query, d->b_g2_query_len, wwb, k, &pk->b_g2));
+  if (nw) CS_TRY(bases_upload(ctx, d->curve, CS_G1, d->l_query, d->l_query_len, wwb, k, &pk->l_query));
+  CS_TRY(bases_upload(ctx, d->curve, CS_G1, d->h_query, n, hwb, k, &pk->h_query));
   CS_TRY(plan_witness_views(ctx, pk.get()));
   switch (d->curve) {
     case CS_BN254: CS_TRY(build_coset_table<Bn254Cfg>(ctx, pk.get())); break;
@@ -746,6 +784,8 @@ int cs_groth16_pk_create(cs_ctx* ctx, const cs_groth16_key_desc* d, cs_groth16_p
   *out = pk.release();
   return 0;
 }
+
+extern "C" {
 
 void cs_groth16_pk_free(cs_groth16_pk* pk) {
   if (!pk) return;
@@ -764,6 +804,17 @@ void cs_groth16_pk_free(cs_groth16_pk* pk) {
 }
 
 size_t cs_groth16_domain_size(const cs_groth16_pk* pk) { return pk ? pk->n : 0; }
+
+int cs_groth16_pk_table_info(const cs_groth16_pk* pk, unsigned* table_rows, size_t* table_bytes) {
+  if (!pk) return fail(CS_ERR_ARG, "cs_groth16_pk_table_info: pk is NULL");
+  const cs_bases* q[5] = {pk->a_query, pk->b_g1, pk->b_g2, pk->l_query, pk->h_query};
+  size_t bytes = 0;
+  for (const cs_bases* b : q)
+    if (b) bytes += b->table.cap + b->infmask.cap;
+  if (table_rows) *table_rows = pk->a_query->sh.T;
+  if (table_bytes) *table_bytes = bytes;
+  return 0;
+}
 int cs_groth16_pk_curve(const cs_groth16_pk* pk) { return pk ? pk->curve : CS_ERR_ARG; }
 
 int cs_groth16_witness_map(cs_ctx* ctx, cs_groth16_pk* pk, cs_share_kind kind, int party, const uint64_t* h_pub,

@@ -1,6 +1,7 @@
 // Library internals shared by the C-ABI translation units: curve configs, context, handles.
 #pragma once
 #include <atomic>
+#include <functional>
 #include <map>
 #include <memory>
 #include "cs_common.cuh"
@@ -63,13 +64,14 @@ struct cs_ctx {
   cs::DevBuf io;  // staging for host-buffer convenience calls
   cs::DevBuf prf_keys;
   cs::DevBuf sc_part, sc_res;  // sumcheck round: per-block partial sums and the 16 results (reused across rounds)
+  size_t table_budget = 0;     // cs_ctx_set_table_budget: cap on the device bytes a new key's tables may take, 0 = none
 };
 
 struct cs_bases {
   int curve = 0, group = 0;
   size_t n = 0;
   cs::MsmShape sh{};
-  cs::DevBuf table;    // W * n affine points
+  cs::DevBuf table;    // T * n affine points: T = sh.T rows of one per sh.k windows
   cs::DevBuf infmask;  // 1 bit per base: point at infinity
   bool m260 = false;   // table coordinates are in the radix-2^260 Montgomery form: accumulate on the FP64 pipe (cs_msm52.cuh)
 };
@@ -116,6 +118,29 @@ int msm_enqueue_dyn(cs_ctx* ctx, int slot, cudaStream_t st, const cs_bases* b, s
 int msm_sort_shared_dyn(cs_ctx* ctx, int slot, cudaStream_t st, const cs_bases* b, const uint32_t* d_scalars,
                         unsigned sstride, size_t n, int mont);
 int msm_finish_dyn(cs_ctx* ctx, int slot, const cs_bases* b, uint64_t* out_affine, int* out_inf);
+
+// widest window an MSM can run: msm_scan takes 2^20 bucket slots, 2^(c-1) buckets plus bucket 0
+constexpr unsigned MSM_MAX_WINDOW = 20;
+static_assert((1u << (MSM_MAX_WINDOW - 1)) + 1 <= MSM_SCAN_MAX_BLOCKS * MSM_SCAN_T, "MSM_MAX_WINDOW exceeds the scan");
+
+// Table rows.  A key's MSM tables keep one row per k windows (MsmShape); k is the smallest whose device bytes fit the
+// budget: what cudaMemGetInfo reports free less TABLE_MARGIN (the CUDA runtime's own allocations), capped by
+// cs_ctx_set_table_budget.  k = 1 (full tables) whenever they fit.
+constexpr size_t TABLE_MARGIN = 256ull << 20;
+int table_budget(cs_ctx* ctx, size_t* out);
+// smallest k in 1..W with need(k) <= budget, or CS_ERR_LIMIT stating the bytes needed at k = W and the budget
+int pick_table_rows(cs_ctx* ctx, unsigned c, unsigned W, const std::function<size_t(unsigned)>& need, const char* who,
+                    unsigned* k_out);
+// device bytes of an uploaded base set of n points in shape sh
+template <class Cfg, int G>
+size_t bases_bytes(size_t n, const MsmShape& sh) {
+  return DevBuf::alloc_size((size_t)sh.T * n * sizeof(Affine<typename GroupOf<Cfg, G>::F>)) + DevBuf::alloc_size(((n + 31) / 32) * 4);
+}
+// cs_bases_upload with k windows per table row, or k = 0: chosen by pick_table_rows for this base set alone
+int bases_upload(cs_ctx* ctx, cs_curve curve, cs_group group, const uint64_t* h_points_mont, size_t n, int window_bits,
+                 unsigned k, cs_bases** out);
+// cs_groth16_pk_create with k windows per table row for all five tables, or k = 0: chosen by pick_table_rows
+int groth16_pk_create(cs_ctx* ctx, const cs_groth16_key_desc* d, unsigned k, cs_groth16_pk** out);
 int ntt_run(cs_ctx* ctx, const cs_domain* d, uint32_t* d_data, unsigned batch, bool inverse_in_to_out,
             const uint32_t* d_post, cudaStream_t st);
 }  // namespace cs

@@ -8,7 +8,8 @@
 //  * The base set is a proving key / SRS: it is uploaded once and expanded to a table of
 //    2^(c w) * P_i for every window w (W x the key size: ~6.4 GB for a 2^20 Groth16 key, which 80 GB of HBM affords).  All
 //    windows then share ONE bucket set, so there is no per-window reduction and no window-combine
-//    doubling chain on the per-proof path.
+//    doubling chain on the per-proof path.  A key whose full tables do not fit keeps one row per k windows and k
+//    bucket groups, combined by c (k - 1) doublings (MsmShape).
 //  * Per MSM: signed c-bit digits -> counting sort by bucket (histogram, scan, scatter) -> bucket
 //    accumulation as a load-balanced segmented reduction over fixed-size slices of the sorted entry
 //    list (robust to skewed scalars) -> weighted bucket reduction sum_b b * S_b.
@@ -26,23 +27,24 @@ constexpr unsigned MSM_RED_SEG = 4;     // buckets per thread in the weighted bu
 constexpr unsigned MSM_SIGN = 0x80000000u;
 
 // --------------------------------------------------------------------------- digits
-// Scalar i: optional Montgomery -> canonical, then signed c-bit recoding; f(w, digit) for every window w, where the
-// digit is bucket | MSM_SIGN and bucket 0 is a zero digit.
+// Scalar i: optional Montgomery -> canonical, then signed c-bit recoding; f(row, digit) for every window w, where the
+// digit is bucket | MSM_SIGN and bucket 0 is a zero digit.  A table of one row per k windows (MsmShape) puts window w
+// in row w / k and its digits d in bucket group w % k: bucket (w % k) B + d.  k = 1: row w, bucket d.
 template <class FrP, class Fn>
 CS_D void msm_recode(const uint32_t* __restrict__ scalars, uint32_t sstride, uint32_t i, int mont, uint32_t c,
-                     uint32_t W, Fn&& f) {
+                     uint32_t W, uint32_t k, Fn&& f) {
   Fp<FrP> s;
   // sstride = elements between consecutive scalars (2 reads the `a` component of Rep3 shares in place)
   const uint4* src = reinterpret_cast<const uint4*>(scalars) + (size_t)i * sstride * (FrP::N / 4);
   CS_UNROLL
-  for (int k = 0; k < FrP::N / 4; k++) {
-    uint4 v = src[k];
-    s.l[4 * k] = v.x; s.l[4 * k + 1] = v.y; s.l[4 * k + 2] = v.z; s.l[4 * k + 3] = v.w;
+  for (int q = 0; q < FrP::N / 4; q++) {
+    uint4 v = src[q];
+    s.l[4 * q] = v.x; s.l[4 * q + 1] = v.y; s.l[4 * q + 2] = v.z; s.l[4 * q + 3] = v.w;
   }
   if (mont) s = s.from_mont();
   const uint32_t half = 1u << (c - 1);
   const uint32_t mask = (1u << c) - 1;
-  uint32_t carry = 0;
+  uint32_t carry = 0, row = 0, gb = 0;  // gb = first bucket of the group - 1
   for (uint32_t w = 0; w < W; w++) {
     uint32_t pos = w * c;
     uint32_t li = pos >> 5, sh = pos & 31;
@@ -51,13 +53,18 @@ CS_D void msm_recode(const uint32_t* __restrict__ scalars, uint32_t sstride, uin
     uint32_t d = (__funnelshift_r(lo, hi, sh) & mask) + carry;
     uint32_t out;
     if (d > half) {
-      out = ((1u << c) - d) | MSM_SIGN;
+      out = ((1u << c) - d) | MSM_SIGN;  // d = 2^c: a zero digit with a carry
       carry = 1;
     } else {
       out = d;
       carry = 0;
     }
-    f(w, out);
+    f(row, out & ~MSM_SIGN ? out + gb : 0);
+    gb += half;
+    if (gb == k * half) {
+      gb = 0;
+      row++;
+    }
   }
 }
 
@@ -88,7 +95,7 @@ constexpr unsigned MSM_SCATTER_SPAN = 1u << 13;  // buckets per grid.y slice of 
 
 template <class FrP>
 CS_GLOBAL void __launch_bounds__(MSM_BIN_T) k_msm_bin_count(const uint32_t* __restrict__ scalars, uint32_t sstride,
-                                                            uint32_t n, int mont, uint32_t c, uint32_t W,
+                                                            uint32_t n, int mont, uint32_t c, uint32_t W, uint32_t kw,
                                                             const uint32_t* __restrict__ infmask, uint32_t offset,
                                                             uint32_t tile, uint32_t B, uint32_t* __restrict__ tab) {
   CS_DYN_SMEM(uint32_t, h);
@@ -99,7 +106,7 @@ CS_GLOBAL void __launch_bounds__(MSM_BIN_T) k_msm_bin_count(const uint32_t* __re
   const uint32_t i1 = (blockIdx.x + 1) * tile < n ? (blockIdx.x + 1) * tile : n;
   for (uint32_t i = blockIdx.x * tile + threadIdx.x; i < i1; i += blockDim.x) {
     if (msm_base_inf(infmask, offset + i)) continue;
-    msm_recode<FrP>(scalars, sstride, i, mont, c, W, [&](uint32_t, uint32_t d) {
+    msm_recode<FrP>(scalars, sstride, i, mont, c, W, kw, [&](uint32_t, uint32_t d) {
       const uint32_t k = (d & ~MSM_SIGN) - lo;  // wraps past span for bucket 0 and for buckets below lo
       if (k < span) atomicAdd(&h[k], 1u);
     });
@@ -135,10 +142,10 @@ static CS_GLOBAL void k_msm_bin_scan(uint32_t* __restrict__ tab, uint32_t nblk, 
   count[b + 1] = run;
 }
 
-// sorted[pos] = table slot w * nbases + offset + i | sign, grouped by bucket
+// sorted[pos] = table slot row * nbases + offset + i | sign, grouped by bucket
 template <class FrP>
 CS_GLOBAL void __launch_bounds__(MSM_BIN_T) k_msm_bin_scatter(const uint32_t* __restrict__ scalars, uint32_t sstride,
-                                                              uint32_t n, int mont, uint32_t c, uint32_t W,
+                                                              uint32_t n, int mont, uint32_t c, uint32_t W, uint32_t kw,
                                                               const uint32_t* __restrict__ infmask, uint32_t offset,
                                                               uint32_t tile, uint32_t B, uint32_t nbases,
                                                               const uint32_t* __restrict__ tab,
@@ -153,9 +160,9 @@ CS_GLOBAL void __launch_bounds__(MSM_BIN_T) k_msm_bin_scatter(const uint32_t* __
   const uint32_t i1 = (blockIdx.x + 1) * tile < n ? (blockIdx.x + 1) * tile : n;
   for (uint32_t i = blockIdx.x * tile + threadIdx.x; i < i1; i += blockDim.x) {
     if (msm_base_inf(infmask, offset + i)) continue;
-    msm_recode<FrP>(scalars, sstride, i, mont, c, W, [&](uint32_t w, uint32_t d) {
+    msm_recode<FrP>(scalars, sstride, i, mont, c, W, kw, [&](uint32_t row, uint32_t d) {
       const uint32_t k = (d & ~MSM_SIGN) - lo;
-      if (k < span) sorted[atomicAdd(&cur[k], 1u)] = (w * nbases + offset + i) | (d & MSM_SIGN);
+      if (k < span) sorted[atomicAdd(&cur[k], 1u)] = (row * nbases + offset + i) | (d & MSM_SIGN);
     });
   }
 }
@@ -255,11 +262,12 @@ static CS_GLOBAL void k_msm_scan2(const uint32_t* __restrict__ count, uint32_t n
 
 // --------------------------------------------------------------------------- filtered view of a shared sort
 // Groth16's A, B1, B2 and L MSMs take the same witness scalars over different tables.  Their digits are sorted ONCE
-// without an infinity mask (msm_sort with infmask = null, entries w * n + i: window w, scalar i); a table with
-// infinity bases, or whose slots are not w * n + i, gets a stream compaction of those entries that drops the entries
-// of its infinite bases and rewrites the rest to its own slots, w * nbases + offset + i.  The compaction keeps the
-// order, so the view is grouped by bucket as the shared entries are, and its bucket counts follow from the kept
-// entries before each shared bucket start: per-block counts and keep bitmaps, no per-entry global atomics.
+// without an infinity mask (msm_sort with infmask = null, entries j * n + i: table row j, scalar i); a table with
+// infinity bases, or whose slots are not j * n + i, gets a stream compaction of those entries that drops the entries
+// of its infinite bases and rewrites the rest to its own slots, j * nbases + offset + i (the tables share one window
+// shape: c, W and windows per row k).  The compaction keeps the order, so the view is grouped by bucket as the shared
+// entries are, and its bucket counts follow from the kept entries before each shared bucket start: per-block counts
+// and keep bitmaps, no per-entry global atomics.
 constexpr unsigned MSM_VIEW_T = 256;  // entries per block of the view kernels, one per thread
 constexpr unsigned MSM_VIEW_WORDS = MSM_VIEW_T / 32;
 
@@ -551,27 +559,29 @@ CS_GLOBAL void __launch_bounds__(128) k_msm_accum2(const Xyzz<F>* __restrict__ p
 }
 
 // --------------------------------------------------------------------------- bucket reduction
-// Thread t owns buckets (t L, (t+1) L]:  out[t] = sum_{b} b * S_b  over its segment
-//   = tot + (t L) * acc,   acc = sum S_b,  tot = sum (b - t L) S_b  by a running sum.
+// Thread t owns buckets (t L, (t+1) L] of the NB = k B buckets:  out[t] = sum_{b} (b - g B) * S_b  over its segment,
+// g = the bucket group (L divides B, so a segment lies in one group)
+//   = tot + (t L - g B) * acc,   acc = sum S_b,  tot = sum (b - t L) S_b  by a running sum.
 template <class F>
-CS_GLOBAL void __launch_bounds__(128) k_msm_reduce_seg(const Xyzz<F>* __restrict__ bucket, uint32_t B,
+CS_GLOBAL void __launch_bounds__(128) k_msm_reduce_seg(const Xyzz<F>* __restrict__ bucket, uint32_t NB, uint32_t B,
                                                        uint32_t L, Xyzz<F>* __restrict__ red) {
   uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
   uint32_t lo = t * L;
-  if (lo >= B) return;
-  uint32_t hi = lo + L < B ? lo + L : B;
+  if (lo >= NB) return;
+  uint32_t hi = lo + L < NB ? lo + L : NB;
+  const uint32_t w = lo & (B - 1);  // t L - g B (B is a power of two)
   Xyzz<F> acc = Xyzz<F>::inf(), tot = Xyzz<F>::inf();
   for (uint32_t b = hi; b > lo; b--) {
     padd(acc, bucket[b]);
     padd(tot, acc);
   }
-  // tot += lo * acc   (double-and-add, lo < 2^31)
-  if (lo != 0 && !acc.is_inf()) {
+  // tot += w * acc   (double-and-add, w < 2^31)
+  if (w != 0 && !acc.is_inf()) {
     Xyzz<F> m = Xyzz<F>::inf();
-    int top = 31 - __clz(lo);
+    int top = 31 - __clz(w);
     for (int bit = top; bit >= 0; bit--) {
       m = dbl_xyzz(m);
-      if ((lo >> bit) & 1) padd(m, acc);
+      if ((w >> bit) & 1) padd(m, acc);
     }
     padd(tot, m);
   }
@@ -581,12 +591,14 @@ CS_GLOBAL void __launch_bounds__(128) k_msm_reduce_seg(const Xyzz<F>* __restrict
 // No warp-shuffle tree here: every lane would pay the full point addition in every round, and moving a 128/256-byte
 // XYZZ point is 32/64 SHFL, so a shuffle tree is slower than the shared-memory tree below.
 // Block b sums red[k] for k = b*T + t, stride gridDim.x*T, into out[b] (shared-memory tree); launched
-// twice: many blocks, then one block over the block results.
+// twice: many blocks, then one block over the block results.  grid.y = bucket groups, each over its own cnt inputs.
 template <class F>
 CS_GLOBAL void k_msm_final_sum(const Xyzz<F>* __restrict__ red, uint32_t cnt,
                                                       Xyzz<F>* __restrict__ out) {
   CS_DYN_SMEM(Xyzz<F>, sm);
   const uint32_t T = blockDim.x, t = threadIdx.x;
+  red += (size_t)blockIdx.y * cnt;
+  out += (size_t)blockIdx.y * gridDim.x;
   Xyzz<F> acc = Xyzz<F>::inf();
   for (uint32_t k = blockIdx.x * T + t; k < cnt; k += gridDim.x * T) padd(acc, red[k]);
   sm[t] = acc;
@@ -600,6 +612,18 @@ CS_GLOBAL void k_msm_final_sum(const Xyzz<F>* __restrict__ red, uint32_t cnt,
     __syncthreads();
   }
   if (t == 0) out[blockIdx.x] = sm[0];
+}
+
+// One thread: the k group sums R_g of a table with one row per k windows -> sum_g 2^(c g) R_g by Horner's rule
+// (c (k - 1) doublings).
+template <class F>
+CS_GLOBAL void k_msm_combine_groups(const Xyzz<F>* __restrict__ gsum, uint32_t k, uint32_t c, Xyzz<F>* __restrict__ out) {
+  Xyzz<F> acc = gsum[k - 1];
+  for (uint32_t g = k - 1; g-- > 0;) {
+    for (uint32_t d = 0; d < c; d++) acc = dbl_xyzz(acc);
+    padd(acc, gsum[g]);
+  }
+  out[0] = acc;
 }
 
 // --------------------------------------------------------------------------- table precomputation
@@ -686,15 +710,22 @@ CS_GLOBAL void __launch_bounds__(128) k_fixed_base_mul(const Affine<F>* __restri
 }
 
 // --------------------------------------------------------------------------- host driver
+// A table keeps one row per k windows, T = ceil(W / k) rows: row j = 2^(c k j) P_i (k_msm_precompute with window c k).
+// Window w reads row w / k and accumulates into bucket group w % k (k B buckets in all); the group sums are combined
+// as sum_g 2^(c g) R_g.  k = 1 is the full table: a row per window and one bucket group.
 struct MsmShape {
-  uint32_t c, W, B;  // window bits, windows, buckets (1..B)
+  uint32_t c, W, B;  // window bits, windows, buckets per group (1..B)
+  uint32_t k = 1, T = 0;  // windows per table row, table rows
+  uint32_t nb() const { return k * B; }  // buckets of all groups (1..k B)
 };
 
-static inline MsmShape msm_shape(uint32_t scalar_bits, uint32_t c) {
+static inline MsmShape msm_shape(uint32_t scalar_bits, uint32_t c, uint32_t k = 1) {
   MsmShape s;
   s.c = c;
   s.W = (scalar_bits + 1 + c - 1) / c;  // top window keeps <= c-1 bits so the signed recoding never overflows
   s.B = 1u << (c - 1);
+  s.k = k < s.W ? k : s.W;
+  s.T = (s.W + s.k - 1) / s.k;
   return s;
 }
 
@@ -770,7 +801,7 @@ struct MsmSizes {
   uint32_t nb1, S, ob;
   size_t nent, max_s0, max_s1, max_s2;
   MsmSizes(const MsmShape& sh, uint32_t n) {
-    nb1 = sh.B + 1;
+    nb1 = sh.nb() + 1;
     nent = (size_t)sh.W * n;
     S = msm_slice(sh);
     max_s0 = nent / S + nb1;
@@ -807,15 +838,15 @@ struct MsmSortBufs {
 
 static inline int msm_check_limits(const MsmShape& sh, uint32_t n, uint32_t nbases) {
   const size_t nent = (size_t)sh.W * n;
-  if (nent >= (1ull << 31) || (size_t)sh.W * nbases >= (1ull << 31))
-    return fail(-3, "msm: W*n = %zu exceeds 2^31 entries", nent);
+  if (nent >= (1ull << 31) || (size_t)sh.T * nbases >= (1ull << 31))
+    return fail(-3, "msm: W*n = %zu entries or T*nbases = %zu table slots exceed 2^31", nent, (size_t)sh.T * nbases);
   return 0;
 }
 
 // count[] -> bucket starts and slice offsets (start, sstart0..2)
-static inline int msm_scan(const MsmSortBufs& q, const MsmSizes& z, uint32_t B, cudaStream_t st) {
+static inline int msm_scan(const MsmSortBufs& q, const MsmSizes& z, uint32_t NB, cudaStream_t st) {
   const uint32_t sb = ceil_div(z.nb1, MSM_SCAN_T);
-  if (sb > MSM_SCAN_MAX_BLOCKS) return fail(-3, "msm: %u buckets exceed the scan's limit", B);
+  if (sb > MSM_SCAN_MAX_BLOCKS) return fail(-3, "msm: %u buckets exceed the scan's limit", NB);
   CS_LAUNCH_SYNC(k_msm_scan1, sb, MSM_SCAN_T, 0, st, q.count, z.nb1, z.S, q.start, q.sstart0, q.sstart1, q.sstart2, q.aux);
   CS_LAUNCH(k_msm_scan2, sb, MSM_SCAN_T, 0, st, q.count, z.nb1, z.S, q.start, q.sstart0, q.sstart1, q.sstart2, q.aux);
   return 0;
@@ -853,14 +884,56 @@ int msm_smem_optin() {
 // Scalars per block of the bucket sort: MSM_BIN_TILE, or more where nblk rows of B counts would exceed the W n words
 // the table has (windows above 16 at small n).  The table then takes at most max(W n, B) words.
 static inline uint32_t msm_bin_tile(const MsmShape& sh, const MsmSizes& z, uint32_t n) {
-  const size_t rows = z.nent / sh.B > 1 ? z.nent / sh.B : 1;
+  const size_t rows = z.nent / sh.nb() > 1 ? z.nent / sh.nb() : 1;
   const size_t nblk = ceil_div(n, MSM_BIN_TILE) < rows ? ceil_div(n, MSM_BIN_TILE) : rows;
   return n ? ceil_div(n, nblk) : 1;
 }
 
-// Digits, bucket sort and slice order of n scalars into ws; the entries index table slots w * nbases + offset + i.
+// Words of ws.dig: msm_sort's per-block count table (or W n words, whichever is larger) and msm_view's keep bitmap
+// and block counts
+static inline size_t msm_sort_dig_words(const MsmShape& sh, const MsmSizes& z, uint32_t n) {
+  const size_t tab_words = (size_t)(n ? ceil_div(n, msm_bin_tile(sh, z, n)) : 0) * sh.nb();
+  return tab_words > z.nent ? tab_words : z.nent;
+}
+static inline size_t msm_view_dig_words(const MsmSizes& z) {
+  const size_t nblk = ceil_div(z.nent, MSM_VIEW_T);
+  return nblk * MSM_VIEW_WORDS + 2 * nblk + 1;
+}
+
+// Bucket reduction tail of msm_enqueue: segments of L buckets (L divides B), then k_msm_final_sum over each group's
+// nseg_g segment sums in fs_blocks blocks; red holds the segment sums, the block sums and, for k > 1, the group sums.
+template <class F>
+struct MsmReduce {
+  uint32_t L, nseg_g, nseg, fs_threads, fs_blocks;
+  size_t red_elems;
+  explicit MsmReduce(const MsmShape& sh) {
+    L = sh.B < MSM_RED_SEG ? sh.B : MSM_RED_SEG;
+    nseg_g = sh.B / L;
+    nseg = sh.k * nseg_g;
+    fs_threads = sizeof(Xyzz<F>) > 128 ? 128 : 256;  // <= 32 KB of dynamic shared memory
+    fs_blocks = nseg_g > 4 * fs_threads ? (nseg_g + fs_threads - 1) / fs_threads : 1;
+    red_elems = (size_t)nseg + (size_t)sh.k * fs_blocks + (sh.k > 1 ? sh.k : 0);
+  }
+};
+
+// Device bytes msm_sort / msm_view (sort) and msm_enqueue (accumulation) reserve in a workspace for n scalars
+static inline size_t msm_sort_bytes(const MsmShape& sh, uint32_t n) {
+  const MsmSizes z(sh, n);
+  const size_t dig = msm_sort_dig_words(sh, z, n) > msm_view_dig_words(z) ? msm_sort_dig_words(sh, z, n) : msm_view_dig_words(z);
+  return DevBuf::alloc_size(dig * 4) + DevBuf::alloc_size(z.nent * 4) + DevBuf::alloc_size(z.meta_words() * 4) +
+         DevBuf::alloc_size(z.order_words() * 4);
+}
+template <class F>
+size_t msm_accum_bytes(const MsmShape& sh, uint32_t n) {
+  const MsmSizes z(sh, n);
+  const size_t x = sizeof(Xyzz<F>);
+  return DevBuf::alloc_size(z.max_s0 * x) + DevBuf::alloc_size(z.max_s1 * x) + DevBuf::alloc_size(z.max_s2 * x) +
+         DevBuf::alloc_size((size_t)z.nb1 * x) + DevBuf::alloc_size(MsmReduce<F>(sh).red_elems * x) + DevBuf::alloc_size(x);
+}
+
+// Digits, bucket sort and slice order of n scalars into ws; the entries index table slots row * nbases + offset + i.
 // infmask = null keeps the entries of every base: with nbases = n and offset = 0 that is the shared witness sort,
-// which msm_enqueue reads as it is (a table without infinity bases and slots w * n + i) or through msm_view.
+// which msm_enqueue reads as it is (a table without infinity bases and slots row * n + i) or through msm_view.
 template <class FrP>
 int msm_sort(MsmWorkspace& ws, const uint32_t* infmask, uint32_t nbases, MsmShape sh, uint32_t offset,
              const uint32_t* d_scalars, uint32_t sstride, uint32_t n, int mont, cudaStream_t st) {
@@ -868,12 +941,12 @@ int msm_sort(MsmWorkspace& ws, const uint32_t* infmask, uint32_t nbases, MsmShap
   const MsmSizes z(sh, n);
   const uint32_t tile = msm_bin_tile(sh, z, n);
   const uint32_t nblk = n ? ceil_div(n, tile) : 0;
-  const dim3 grid(nblk, ceil_div(sh.B, MSM_BIN_SPAN)), grid_sc(nblk, ceil_div(sh.B, MSM_SCATTER_SPAN));
-  const uint32_t smem = (sh.B < MSM_BIN_SPAN ? sh.B : MSM_BIN_SPAN) * 4;
-  const uint32_t smem_sc = (sh.B < MSM_SCATTER_SPAN ? sh.B : MSM_SCATTER_SPAN) * 4;
+  const uint32_t NB = sh.nb();
+  const dim3 grid(nblk, ceil_div(NB, MSM_BIN_SPAN)), grid_sc(nblk, ceil_div(NB, MSM_SCATTER_SPAN));
+  const uint32_t smem = (NB < MSM_BIN_SPAN ? NB : MSM_BIN_SPAN) * 4;
+  const uint32_t smem_sc = (NB < MSM_SCATTER_SPAN ? NB : MSM_SCATTER_SPAN) * 4;
   // dig holds the per-block count table (k_msm_bin_*)
-  const size_t tab_words = (size_t)nblk * sh.B;
-  CS_TRY(ws.dig.reserve((tab_words > z.nent ? tab_words : z.nent) * 4));
+  CS_TRY(ws.dig.reserve(msm_sort_dig_words(sh, z, n) * 4));
   CS_TRY(ws.sorted.reserve(z.nent * 4));
   CS_TRY(ws.meta.reserve(z.meta_words() * 4));
   CS_TRY(ws.order.reserve(z.order_words() * 4));
@@ -881,25 +954,25 @@ int msm_sort(MsmWorkspace& ws, const uint32_t* infmask, uint32_t nbases, MsmShap
   uint32_t* tab = ws.dig.as<uint32_t>();
   CS_TRY(ws.mark(0, st));
   if (nblk)
-    CS_LAUNCH_SYNC(k_msm_bin_count<FrP>, grid, MSM_BIN_T, smem, st, d_scalars, sstride, n, mont, sh.c, sh.W, infmask,
-                   offset, tile, sh.B, tab);
+    CS_LAUNCH_SYNC(k_msm_bin_count<FrP>, grid, MSM_BIN_T, smem, st, d_scalars, sstride, n, mont, sh.c, sh.W, sh.k,
+                   infmask, offset, tile, NB, tab);
   CS_TRY(ws.mark(1, st));
-  CS_LAUNCH(k_msm_bin_scan, ceil_div(sh.B, 256), 256, 0, st, tab, nblk, sh.B, q.count);
-  CS_TRY(msm_scan(q, z, sh.B, st));
+  CS_LAUNCH(k_msm_bin_scan, ceil_div(NB, 256), 256, 0, st, tab, nblk, NB, q.count);
+  CS_TRY(msm_scan(q, z, NB, st));
   if (nblk)
-    CS_LAUNCH_SYNC(k_msm_bin_scatter<FrP>, grid_sc, MSM_BIN_T, smem_sc, st, d_scalars, sstride, n, mont, sh.c, sh.W, infmask,
-                   offset, tile, sh.B, nbases, tab, q.start, ws.sorted.as<uint32_t>());
+    CS_LAUNCH_SYNC(k_msm_bin_scatter<FrP>, grid_sc, MSM_BIN_T, smem_sc, st, d_scalars, sstride, n, mont, sh.c, sh.W, sh.k,
+                   infmask, offset, tile, NB, nbases, tab, q.start, ws.sorted.as<uint32_t>());
   return msm_slice_order(ws, q, z, st);
 }
 
 // This table's entries out of the shared witness sort in src (k_msm_view_*): entries of its infinite bases dropped,
-// the others rewritten to its slots w * nbases + offset + i; then bucket offsets and a slice order of its own.
+// the others rewritten to its slots row * nbases + offset + i; then bucket offsets and a slice order of its own.
 static inline int msm_view(MsmWorkspace& ws, const MsmWorkspace& src, const uint32_t* infmask, uint32_t nbases,
                            MsmShape sh, uint32_t offset, uint32_t n, cudaStream_t st) {
   const MsmSizes z(sh, n);
   const uint32_t nblk = ceil_div(z.nent, MSM_VIEW_T);
   // dig: keep bitmap | blk_cnt[nblk] | blk_off[nblk + 1]
-  CS_TRY(ws.dig.reserve(((size_t)nblk * MSM_VIEW_WORDS + 2 * (size_t)nblk + 1) * 4));
+  CS_TRY(ws.dig.reserve(msm_view_dig_words(z) * 4));
   CS_TRY(ws.sorted.reserve(z.nent * 4));
   CS_TRY(ws.meta.reserve(z.meta_words() * 4));
   CS_TRY(ws.order.reserve(z.order_words() * 4));
@@ -913,7 +986,7 @@ static inline int msm_view(MsmWorkspace& ws, const MsmWorkspace& src, const uint
   CS_LAUNCH(k_msm_view_counts, ceil_div(z.nb1, 256), 256, 0, st, s.start, z.nb1, keep, blk_off, q.count);
   CS_LAUNCH(k_msm_view_scatter, nblk, MSM_VIEW_T, 0, st, src_sorted, n, nbases, offset, keep, blk_off,
             ws.sorted.as<uint32_t>());
-  CS_TRY(msm_scan(q, z, sh.B, st));
+  CS_TRY(msm_scan(q, z, sh.nb(), st));
   return msm_slice_order(ws, q, z, st);
 }
 
@@ -942,11 +1015,9 @@ int msm_enqueue(MsmWorkspace& ws, const Affine<F>* table, const uint32_t* infmas
   CS_TRY(ws.part1.reserve(max_s1 * sizeof(Xyzz<F>)));
   CS_TRY(ws.part2.reserve(max_s2 * sizeof(Xyzz<F>)));
   CS_TRY(ws.bucket.reserve((size_t)nb1 * sizeof(Xyzz<F>)));
-  const uint32_t L = sh.B < MSM_RED_SEG ? sh.B : MSM_RED_SEG;
-  const uint32_t nseg = (sh.B + L - 1) / L;
-  const uint32_t fs_threads = sizeof(Xyzz<F>) > 128 ? 128 : 256;  // <= 32 KB of dynamic shared memory
-  const uint32_t fs_blocks = nseg > 4 * fs_threads ? (nseg + fs_threads - 1) / fs_threads : 1;
-  CS_TRY(ws.red.reserve(((size_t)nseg + fs_blocks) * sizeof(Xyzz<F>)));
+  const MsmReduce<F> rd(sh);
+  const uint32_t L = rd.L, nseg = rd.nseg, fs_threads = rd.fs_threads, fs_blocks = rd.fs_blocks;
+  CS_TRY(ws.red.reserve(rd.red_elems * sizeof(Xyzz<F>)));
   CS_TRY(ws.result.reserve(sizeof(Xyzz<F>)));
   if (ws.h_result_cap < sizeof(Xyzz<F>)) {
     if (ws.h_result) cudaFreeHost(ws.h_result);
@@ -1013,18 +1084,21 @@ int msm_enqueue(MsmWorkspace& ws, const Affine<F>* table, const uint32_t* infmas
   CS_LAUNCH(k_msm_accum2<F>, ceil_div(nb1, 128), 128, 0, st, ws.part2.as<Xyzz<F>>(), sstart2, nb1,
             ws.bucket.as<Xyzz<F>>());
   CS_TRY(ws.mark(4, st));
-  CS_LAUNCH(k_msm_reduce_seg<F>, ceil_div(nseg, 128), 128, 0, st, ws.bucket.as<Xyzz<F>>(), sh.B, L,
+  CS_LAUNCH(k_msm_reduce_seg<F>, ceil_div(nseg, 128), 128, 0, st, ws.bucket.as<Xyzz<F>>(), sh.nb(), sh.B, L,
             ws.red.as<Xyzz<F>>());
+  // one sum per bucket group: the MSM result itself when k = 1, else the group sums that k_msm_combine_groups weights
+  Xyzz<F>* gsum = sh.k > 1 ? ws.red.as<Xyzz<F>>() + nseg + (size_t)sh.k * fs_blocks : ws.result.as<Xyzz<F>>();
   if (fs_blocks > 1) {
     Xyzz<F>* stage = ws.red.as<Xyzz<F>>() + nseg;
-    CS_LAUNCH_SYNC(k_msm_final_sum<F>, fs_blocks, fs_threads, fs_threads * sizeof(Xyzz<F>), st, ws.red.as<Xyzz<F>>(), nseg,
-                   stage);
-    CS_LAUNCH_SYNC(k_msm_final_sum<F>, 1, fs_threads, fs_threads * sizeof(Xyzz<F>), st, stage, fs_blocks,
-                   ws.result.as<Xyzz<F>>());
+    CS_LAUNCH_SYNC(k_msm_final_sum<F>, dim3(fs_blocks, sh.k), fs_threads, fs_threads * sizeof(Xyzz<F>), st,
+                   ws.red.as<Xyzz<F>>(), rd.nseg_g, stage);
+    CS_LAUNCH_SYNC(k_msm_final_sum<F>, dim3(1, sh.k), fs_threads, fs_threads * sizeof(Xyzz<F>), st, stage, fs_blocks, gsum);
   } else {
-    CS_LAUNCH_SYNC(k_msm_final_sum<F>, 1, fs_threads, fs_threads * sizeof(Xyzz<F>), st, ws.red.as<Xyzz<F>>(), nseg,
-                   ws.result.as<Xyzz<F>>());
+    CS_LAUNCH_SYNC(k_msm_final_sum<F>, dim3(1, sh.k), fs_threads, fs_threads * sizeof(Xyzz<F>), st, ws.red.as<Xyzz<F>>(),
+                   rd.nseg_g, gsum);
   }
+  if (sh.k > 1)
+    CS_LAUNCH(k_msm_combine_groups<F>, 1, 1, 0, st, gsum, sh.k, sh.c, ws.result.as<Xyzz<F>>());
   CS_TRY(ws.mark(5, st));
   CS_CUDA(cudaMemcpyAsync(ws.h_result, ws.result.p, sizeof(Xyzz<F>), cudaMemcpyDeviceToHost, st));
   CS_CUDA(cudaGetLastError());

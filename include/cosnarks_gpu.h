@@ -71,9 +71,14 @@ int cs_memcpy_d2h(cs_ctx* ctx, void* h_dst, const void* d_src, size_t bytes);
  * co-noir/co-noir-common/src/honk_curve.rs:81-83.
  *
  * cs_bases_upload: upload `n` affine points (Montgomery) once per proving key / SRS; the library
- * expands them into the per-window table it keeps resident in HBM.  window_bits = 0 picks a default
- * (at most 16); an explicit window_bits must lie in [2, 20], the widest window the bucket sort takes, and
- * anything else fails here with CS_ERR_ARG (so does a Groth16 key created with such a window).
+ * expands them into a table of multiples 2^(c k j) P_i it keeps resident in HBM, one row j per k of the W
+ * windows (T = ceil(W / k) rows; the reference keeps only the points and doubles per window on every MSM).
+ * k is the smallest whose table fits the table budget: what the device reports free at creation, less a
+ * small margin, capped by cs_ctx_set_table_budget.  k = 1 (a row per window: the fastest MSM) whenever it
+ * fits; a base set that does not fit even as one row fails with CS_ERR_LIMIT.  The MSM result does not
+ * depend on k.  window_bits = 0 picks a default (at most 16); an explicit window_bits must lie in [2, 20],
+ * the widest window the bucket sort takes, and anything else fails here with CS_ERR_ARG (so does a
+ * Groth16 key created with such a window).
  * cs_msm: sum_{i<n} scalars[i] * bases[offset + i]; the reference "chops to the shorter slice"
  * (honk_curve.rs:33-34) -- pass n = min(len).  scalars_montgomery = 1 for `&[Fr]` (msm_unchecked),
  * 0 for canonical `&[BigInt]` (msm_bigint; must be < r).  Result: affine point (Montgomery), all-zero
@@ -82,6 +87,14 @@ int cs_bases_upload(cs_ctx* ctx, cs_curve curve, cs_group group, const uint64_t*
                     int window_bits, cs_bases** out);
 void cs_bases_free(cs_bases* bases);
 size_t cs_bases_len(const cs_bases* bases);
+/* shape of an uploaded base set: window bits c, windows W, table rows T, and the device bytes it holds;
+ * any output pointer may be NULL */
+int cs_bases_info(const cs_bases* bases, unsigned* window_bits, unsigned* windows, unsigned* table_rows,
+                  size_t* device_bytes);
+/* Cap on the device bytes a base set or key created on this context may take (its tables and, for a
+ * Groth16 key, the scratch its proofs reserve); 0 = automatic: what the device has free.  For callers
+ * that keep several keys on one GPU (e.g. three Rep3 parties), which the library cannot see coming. */
+int cs_ctx_set_table_budget(cs_ctx* ctx, size_t bytes);
 int cs_msm(cs_ctx* ctx, const cs_bases* bases, size_t offset, const uint64_t* h_scalars, size_t n,
            int scalars_montgomery, uint64_t* h_out_affine_mont, int* out_is_infinity);
 int cs_msm_device(cs_ctx* ctx, const cs_bases* bases, size_t offset, const uint64_t* d_scalars, size_t n,
@@ -201,6 +214,9 @@ typedef struct {
 int cs_groth16_pk_create(cs_ctx* ctx, const cs_groth16_key_desc* desc, cs_groth16_pk** out);
 void cs_groth16_pk_free(cs_groth16_pk* pk);
 size_t cs_groth16_domain_size(const cs_groth16_pk* pk);
+/* the key's MSM tables: rows per table (W when every window has its own row; fewer when the tables had to
+ * be compacted to fit, see cs_bases_upload) and their device bytes; either output pointer may be NULL */
+int cs_groth16_pk_table_info(const cs_groth16_pk* pk, unsigned* table_rows, size_t* table_bytes);
 /* the curve the key was built for (cs_curve; read from the zkey's base-field modulus by cs_groth16_pk_from_zkey) */
 int cs_groth16_pk_curve(const cs_groth16_pk* pk);
 

@@ -68,6 +68,9 @@ extern "C" {
     pub fn cs_bases_upload(ctx: *mut cs_ctx, curve: c_int, group: c_int, pts: *const u64, n: usize,
                            window_bits: c_int, out: *mut *mut cs_bases) -> c_int;
     pub fn cs_bases_free(b: *mut cs_bases);
+    pub fn cs_bases_info(b: *const cs_bases, window_bits: *mut c_uint, windows: *mut c_uint, table_rows: *mut c_uint,
+                         device_bytes: *mut usize) -> c_int;
+    pub fn cs_ctx_set_table_budget(ctx: *mut cs_ctx, bytes: usize) -> c_int;
     pub fn cs_msm(ctx: *mut cs_ctx, b: *const cs_bases, offset: usize, scalars: *const u64, n: usize,
                   scalars_montgomery: c_int, out_affine: *mut u64, out_is_inf: *mut c_int) -> c_int;
     pub fn cs_domain_create(ctx: *mut cs_ctx, curve: c_int, log_n: c_uint, gen: *const u64,
@@ -79,6 +82,7 @@ extern "C" {
     pub fn cs_groth16_pk_create(ctx: *mut cs_ctx, d: *const cs_groth16_key_desc, out: *mut *mut cs_groth16_pk) -> c_int;
     pub fn cs_groth16_pk_free(pk: *mut cs_groth16_pk);
     pub fn cs_groth16_domain_size(pk: *const cs_groth16_pk) -> usize;
+    pub fn cs_groth16_pk_table_info(pk: *const cs_groth16_pk, table_rows: *mut c_uint, table_bytes: *mut usize) -> c_int;
     pub fn cs_groth16_witness_map(ctx: *mut cs_ctx, pk: *mut cs_groth16_pk, kind: c_int, party: c_int,
                                   public_inputs: *const u64, witness: *const u64, mask1: *const u64,
                                   mask2: *const u64, h_out: *mut u64) -> c_int;

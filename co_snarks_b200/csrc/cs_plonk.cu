@@ -21,6 +21,42 @@ template <class Cfg>
 int eval_poly_t(cs_ctx* ctx, const uint64_t* d_coeffs, size_t n, unsigned batch, const uint64_t* h_point, uint64_t* h_out);
 }
 
+namespace {
+
+// One prover's per-proof device workspace, reserved once: the plain prover's in the key, each party's in its session.
+// w, buf, poly and ev hold `comps` field elements per entry (1: values or Shamir shares, 2: Rep3 share pairs); the
+// quotient and opening vectors t .. tmp1 hold one.
+struct PlonkWork {
+  DevBuf w, buf[3], poly[4], ev[4], t, tz, t1, t2, t3, tmp0, tmp1, totals, small;
+
+  int reserve(size_t n, size_t n_vars, size_t comps) {
+    CS_TRY(w.reserve(n_vars * comps * 32));
+    for (DevBuf& b : buf) CS_TRY(b.reserve(n * comps * 32));
+    for (int i = 0; i < 4; i++) {
+      CS_TRY(poly[i].reserve((n + 8) * comps * 32));
+      CS_TRY(ev[i].reserve(4 * n * comps * 32));
+    }
+    CS_TRY(t.reserve(4 * n * 32));
+    CS_TRY(tz.reserve(4 * n * 32));
+    for (DevBuf* b : {&t1, &t2, &t3, &tmp0, &tmp1}) CS_TRY(b->reserve((n + 8) * 32));
+    return small.reserve(8192);  // divide_by_linear's table, then r3_batch_inverse's inverse at 4 KB
+  }
+  std::vector<const DevBuf*> all() const {
+    return {&w, &buf[0], &buf[1], &buf[2], &poly[0], &poly[1], &poly[2], &poly[3], &ev[0], &ev[1], &ev[2], &ev[3],
+            &t, &tz, &t1, &t2, &t3, &tmp0, &tmp1, &totals, &small};
+  }
+  void release() {
+    for (const DevBuf* b : all()) const_cast<DevBuf*>(b)->release();
+  }
+  size_t bytes() const {
+    size_t s = 0;
+    for (const DevBuf* b : all()) s += b->cap;
+    return s;
+  }
+};
+
+}  // namespace
+
 struct cs_plonk_pk {
   int curve = 0;
   uint32_t n_vars = 0, n_public = 0, n = 0, n_additions = 0, n_constraints = 0, nlag = 0;
@@ -32,8 +68,9 @@ struct cs_plonk_pk {
   std::vector<uint32_t> level_ends;  // additions sorted by dependency level
   DevBuf map_a, map_b, map_c;
   DevBuf q_coeffs[5], q_evals[5], s_coeffs[3], s_evals[3], lagrange;
-  // per-proof workspace (allocated once)
-  DevBuf w, buf[3], poly[4], ev[4], t, tz, t1, t2, t3, tmp0, tmp1, totals, small;
+  PlonkWork ws;  // the plain prover's
+
+  uint32_t n_witness() const { return n_vars - n_additions - n_public - 1; }  // private inputs: no leading one, no additions
 };
 
 namespace {
@@ -118,16 +155,16 @@ int upload(cs_ctx* ctx, DevBuf& buf, const void* src, size_t bytes) {
 template <class HR>
 void put(uint32_t* dst, const HR& v) { memcpy(dst, v.l, sizeof(v.l)); }
 
-// H: anything with DevBuf members `totals` and `small` (the key's or a Rep3 session's scratch)
-template <class FrP, int OP, class H>
-int scan(cs_ctx* ctx, H* pk, const uint32_t* in, uint32_t* out, uint32_t n, int rev) {
+// scratch: the workspace's `totals`
+template <class FrP, int OP>
+int scan(cs_ctx* ctx, PlonkWork& ws, const uint32_t* in, uint32_t* out, uint32_t n, int rev) {
   const uint32_t nb = ceil_div(n, SCAN_TILE);
-  CS_TRY(pk->totals.reserve((size_t)nb * 32));
-  CS_LAUNCH_SYNC(k_scan_block<FrP COMMA OP>, nb, SCAN_THREADS, (size_t)SCAN_THREADS * 32, ctx->stream, in, out, n, rev,
-                 pk->totals.template as<uint32_t>());
+  CS_TRY(ws.totals.reserve((size_t)nb * 32));
+  uint32_t* totals = ws.totals.as<uint32_t>();
+  CS_LAUNCH_SYNC(k_scan_block<FrP COMMA OP>, nb, SCAN_THREADS, (size_t)SCAN_THREADS * 32, ctx->stream, in, out, n, rev, totals);
   if (nb > 1) {
-    CS_LAUNCH_SYNC(k_scan_totals<FrP COMMA OP>, 1, 256, (size_t)256 * 32, ctx->stream, pk->totals.template as<uint32_t>(), nb);
-    CS_LAUNCH(k_scan_apply<FrP COMMA OP>, ceil_div(n, 256), 256, 0, ctx->stream, out, n, rev, pk->totals.template as<uint32_t>());
+    CS_LAUNCH_SYNC(k_scan_totals<FrP COMMA OP>, 1, 256, (size_t)256 * 32, ctx->stream, totals, nb);
+    CS_LAUNCH(k_scan_apply<FrP COMMA OP>, ceil_div(n, 256), 256, 0, ctx->stream, out, n, rev, totals);
   }
   CS_CUDA(cudaGetLastError());
   return 0;
@@ -254,29 +291,15 @@ int plonk_pk_create_t(cs_ctx* ctx, const cs_plonk_key_desc* d, cs_plonk_pk* pk) 
     CS_TRY(upload(ctx, pk->s_evals[i], d->s_evals[i], (size_t)4 * n * 32));
   }
   CS_TRY(upload(ctx, pk->lagrange, d->lagrange_evals, (size_t)pk->nlag * 4 * n * 32));
-  // workspace
-  CS_TRY(pk->w.reserve((size_t)d->n_vars * 32));
-  for (int i = 0; i < 3; i++) CS_TRY(pk->buf[i].reserve((size_t)n * 32));
-  for (int i = 0; i < 4; i++) {
-    CS_TRY(pk->poly[i].reserve((size_t)(n + 8) * 32));
-    CS_TRY(pk->ev[i].reserve((size_t)4 * n * 32));
-  }
-  CS_TRY(pk->t.reserve((size_t)4 * n * 32));
-  CS_TRY(pk->tz.reserve((size_t)4 * n * 32));
-  CS_TRY(pk->t1.reserve((size_t)(n + 8) * 32));
-  CS_TRY(pk->t2.reserve((size_t)(n + 8) * 32));
-  CS_TRY(pk->t3.reserve((size_t)(n + 8) * 32));
-  CS_TRY(pk->tmp0.reserve((size_t)(n + 8) * 32));
-  CS_TRY(pk->tmp1.reserve((size_t)(n + 8) * 32));
-  CS_TRY(pk->small.reserve(4096));
+  CS_TRY(pk->ws.reserve(n, d->n_vars, 1));
   CS_CUDA(cudaStreamSynchronize(ctx->stream));
   (void)maxl;
   return 0;
 }
 
 // q(X) = p(X) / (X - x) in place over `p` (len entries -> len - 1), optionally subtracting *sub0 from p[0] first
-template <class Cfg, class H>
-int divide_by_linear(cs_ctx* ctx, H* pk, uint32_t* p, uint32_t len, const host::HFp<typename Cfg::FrP>& x,
+template <class Cfg>
+int divide_by_linear(cs_ctx* ctx, PlonkWork& ws, uint32_t* p, uint32_t len, const host::HFp<typename Cfg::FrP>& x,
                      const host::HFp<typename Cfg::FrP>* sub0) {
   typedef typename Cfg::FrP FrP;
   typedef host::HFp<FrP> HR;
@@ -285,13 +308,13 @@ int divide_by_linear(cs_ctx* ctx, H* pk, uint32_t* p, uint32_t len, const host::
   HR a = x, b = x.inverse();
   for (int j = 0; j < 33; j++) { tab[j] = a; tab[33 + j] = b; a = a.sqr(); b = b.sqr(); }
   if (sub0) tab[66] = *sub0;
-  uint32_t* d_tab = pk->small.template as<uint32_t>();
+  uint32_t* d_tab = ws.small.as<uint32_t>();
   CS_CUDA(cudaMemcpyAsync(d_tab, tab.data(), tab.size() * sizeof(HR), cudaMemcpyHostToDevice, ctx->stream));
   CS_CUDA(cudaStreamSynchronize(ctx->stream));  // `tab` is a stack-owned vector
   const unsigned blocks = ceil_div(ceil_div(len, 8), 128);
   CS_LAUNCH(k_scale_by_powers<FrP>, blocks, 128, 0, ctx->stream, p, d_tab, 0u, 0, sub0 ? d_tab + 66 * FrP::N : (const uint32_t*)nullptr,
             len, p);
-  CS_TRY((scan<FrP, 1>(ctx, pk, p, p, len, 0)));
+  CS_TRY((scan<FrP, 1>(ctx, ws, p, p, len, 0)));
   CS_LAUNCH(k_scale_by_powers<FrP>, blocks, 128, 0, ctx->stream, p, d_tab + 33 * FrP::N, 1u, 1, (const uint32_t*)nullptr, len - 1, p);
   CS_CUDA(cudaGetLastError());
   return 0;
@@ -313,6 +336,13 @@ int quotient_consts(int curve, PlonkConsts& K) {
   return 0;
 }
 
+template <class Cfg>
+host::HFp<typename Cfg::FrP> domain_gen(const cs_plonk_pk* pk) {  // w_n, the generator of the n-point domain
+  host::HFp<typename Cfg::FrP> w;
+  memcpy(w.l, pk->dom->group_gen.data(), sizeof(w.l));
+  return w;
+}
+
 // Round 5's scalars (round5.rs:284-340; calculate_lagrange_evaluations / calculate_pi, lib.rs:181-219): the weights of
 // the linearisation polynomial's terms.  pub: the key's n_public public inputs without the leading slot; ev: the opened
 // eval_a eval_b eval_c eval_s1 eval_s2 eval_zw; beta, gamma, alpha, alpha2, k1, k2 are read from K.
@@ -326,8 +356,7 @@ int lin_weights(const cs_plonk_pk* pk, const uint64_t* pub, const PlonkConsts& K
   HR v[5];
   v[0] = v0;
   for (int i = 1; i < 5; i++) v[i] = v[i - 1] * v[0];
-  HR w_n;
-  memcpy(w_n.l, pk->dom->group_gen.data(), sizeof(w_n.l));
+  const HR w_n = domain_gen<Cfg>(pk);
   HR xin = xi;
   for (unsigned q = 0; q < pk->log_n; q++) xin = xin.sqr();
   const HR zh = xin - HR::one();
@@ -361,154 +390,261 @@ int lin_weights(const cs_plonk_pk* pk, const uint64_t* pub, const PlonkConsts& K
   return 0;
 }
 
+// the commitments of p[0..k) (at most three), `len` coefficients each, into k consecutive points at `out`
+template <class Cfg>
+int commit_polys(cs_ctx* ctx, cs_plonk_pk* pk, const DevBuf* p, int k, size_t len, uint64_t* out) {
+  Commit c[3];
+  for (int i = 0; i < k; i++) c[i] = Commit{p[i].as<uint32_t>(), len, out + i * point_limbs64(pk->curve, CS_G1)};
+  return commit_many<Cfg>(ctx, pk, c, k);
+}
+
+// The Fiat-Shamir challenges of rounds 2-5 (round2.rs:226-245, round3.rs:560-610, round4.rs:108-165, round5.rs:284-340),
+// each the Keccak hash of its own transcript.  What enters each transcript, and in which order, is the protocol's format.
+template <class Cfg>
+struct Challenges {
+  typedef host::HFp<typename Cfg::FrP> HR;
+  static constexpr size_t PL = 2 * host::HFp<typename Cfg::FqP>::N;  // limbs of an affine G1 point
+  HR beta, gamma, alpha, xi, v;
+
+  void round2(const cs_plonk_pk* pk, const uint64_t* pub, const uint64_t* abc) {  // pub: with the leading slot
+    Transcript<Cfg> t;
+    for (int i = 0; i < 8; i++) t.add_point(pk->vk_points.data() + i * PL);
+    for (uint32_t i = 1; i <= pk->n_public; i++) {
+      HR x;
+      memcpy(x.l, pub + (size_t)i * HR::N, sizeof(x.l));
+      t.add_scalar(x);
+    }
+    for (int i = 0; i < 3; i++) t.add_point(abc + i * PL);
+    beta = t.get_challenge();
+    Transcript<Cfg> tg;
+    tg.add_scalar(beta);
+    gamma = tg.get_challenge();
+  }
+  void round3(const uint64_t* z) {
+    Transcript<Cfg> t;
+    t.add_scalar(beta);
+    t.add_scalar(gamma);
+    t.add_point(z);
+    alpha = t.get_challenge();
+  }
+  void round4(const uint64_t* t123) {
+    Transcript<Cfg> t;
+    t.add_scalar(alpha);
+    for (int i = 0; i < 3; i++) t.add_point(t123 + i * PL);
+    xi = t.get_challenge();
+  }
+  void round5(const HR* ev) {  // ev: the opened a b c s1 s2 zw
+    Transcript<Cfg> t;
+    t.add_scalar(xi);
+    for (int i = 0; i < 6; i++) t.add_scalar(ev[i]);
+    v = t.get_challenge();
+  }
+};
+
+// Init round (round1.rs:191-252): w = 0 | public inputs | witness | additions, `comps` elements per variable.  The public
+// values go into component pub_comp, or nowhere when it is negative (Rep3 promote_to_trivial_share,
+// rep3/arithmetic.rs:41-50); the leading one reads as zero (types.rs:118-120).
+template <class Cfg>
+int load_witness(cs_ctx* ctx, const cs_plonk_pk* pk, PlonkWork& ws, const uint64_t* h_pub, const uint64_t* h_wit,
+                 unsigned comps, int pub_comp) {
+  typedef typename Cfg::FrP FrP;
+  constexpr int NW = FrP::N, N = host::HFp<FrP>::N;
+  cudaStream_t st = ctx->stream;
+  const uint32_t npub = pk->n_public, n_priv = pk->n_witness();
+  uint32_t* w = ws.w.as<uint32_t>();
+  std::vector<uint64_t> stage;
+  if (comps == 1 && pub_comp == 0) {  // the caller's layout: copy the public inputs as they are
+    CS_CUDA(cudaMemsetAsync(w, 0, 32, st));
+    if (npub) CS_CUDA(cudaMemcpyAsync(w + NW, h_pub + N, (size_t)npub * 32, cudaMemcpyHostToDevice, st));
+  } else {
+    stage.assign((size_t)(npub + 1) * comps * N, 0);
+    for (uint32_t j = 1; j <= npub && pub_comp >= 0; j++)
+      memcpy(&stage[((size_t)j * comps + pub_comp) * N], h_pub + (size_t)j * N, N * 8);
+    CS_CUDA(cudaMemcpyAsync(w, stage.data(), stage.size() * 8, cudaMemcpyHostToDevice, st));
+  }
+  if (n_priv)
+    CS_CUDA(cudaMemcpyAsync(w + (size_t)(npub + 1) * comps * NW, h_wit, (size_t)n_priv * comps * 32, cudaMemcpyHostToDevice, st));
+  if (!stage.empty()) CS_CUDA(cudaStreamSynchronize(st));  // `stage` is a local vector
+  uint32_t lo = 0;
+  for (uint32_t hi : pk->level_ends) {
+    CS_LAUNCH(k_plonk_additions<FrP>, ceil_div(hi - lo, 128), 128, 0, st, pk->add_order.as<uint32_t>(), lo, hi,
+              pk->add_ids.as<uint32_t>(), pk->add_factors.as<uint32_t>(), pk->n_vars - pk->n_additions, (uint32_t)comps, w);
+    lo = hi;
+  }
+  return 0;
+}
+
+// Round 1 for wire k (round1.rs:108-189, 255-320): gathered from w into buf[k]; poly[k] = its coefficients blinded by
+// b[0], b[1] (`comps` components each, component-major); ev[k] = the 4n-point evaluations of the unblinded polynomial
+template <class Cfg>
+int wire_poly(cs_ctx* ctx, cs_plonk_pk* pk, PlonkWork& ws, int k, unsigned comps, const host::HFp<typename Cfg::FrP>* b) {
+  const uint32_t n = pk->n;
+  const DevBuf* maps[3] = {&pk->map_a, &pk->map_b, &pk->map_c};
+  uint32_t *buf = ws.buf[k].as<uint32_t>(), *poly = ws.poly[k].as<uint32_t>();
+  CS_LAUNCH(k_plonk_gather<typename Cfg::FrP>, ceil_div(n, 256), 256, 0, ctx->stream, maps[k]->as<uint32_t>(), pk->n_constraints,
+            n, (uint32_t)comps, ws.w.as<uint32_t>(), buf);
+  CS_CUDA(cudaMemcpyAsync(poly, buf, (size_t)n * comps * 32, cudaMemcpyDeviceToDevice, ctx->stream));
+  CS_TRY(interpolate_and_extend<Cfg>(ctx, pk, poly, ws.ev[k].as<uint32_t>(), comps));
+  return blind<Cfg>(ctx, poly, n, b, 2, comps);
+}
+
+// Z from its n values in poly[3] (round2.rs:197-250): coefficients blinded by b[0..3), and ev[3] = the 4n-point
+// evaluations of the unblinded polynomial
+template <class Cfg>
+int z_poly(cs_ctx* ctx, cs_plonk_pk* pk, PlonkWork& ws, unsigned comps, const host::HFp<typename Cfg::FrP>* b) {
+  CS_TRY(interpolate_and_extend<Cfg>(ctx, pk, ws.poly[3].as<uint32_t>(), ws.ev[3].as<uint32_t>(), comps));
+  return blind<Cfg>(ctx, ws.poly[3].as<uint32_t>(), pk->n, b, 3, comps);
+}
+
+// K before the challenges: the eleven blinders b[0], b[stride], .. (a Rep3 pair's additive half at stride 2), k1, k2
+template <class Cfg>
+void init_consts(PlonkConsts& K, const cs_plonk_pk* pk, const host::HFp<typename Cfg::FrP>* b, int stride) {
+  memset(&K, 0, sizeof(K));
+  for (int i = 0; i < 11; i++) put(K.b[i], b[stride * i]);
+  memcpy(K.k1, pk->k1.data(), sizeof(K.k1));
+  memcpy(K.k2, pk->k2.data(), sizeof(K.k2));
+}
+
+template <class Cfg>
+int set_alpha(const cs_plonk_pk* pk, PlonkConsts& K, const host::HFp<typename Cfg::FrP>& alpha) {
+  put(K.alpha, alpha);
+  put(K.alpha2, alpha.sqr());
+  return quotient_consts<Cfg>(pk->curve, K);
+}
+
+// the round kernels' views of the key and the workspace
+R3Round2In r3_round2_in(const cs_plonk_pk* pk, const PlonkWork& ws) {
+  return R3Round2In{ws.buf[0].as<uint32_t>(),     ws.buf[1].as<uint32_t>(),     ws.buf[2].as<uint32_t>(),
+                    pk->s_evals[0].as<uint32_t>(), pk->s_evals[1].as<uint32_t>(), pk->s_evals[2].as<uint32_t>(),
+                    pk->dom4->tw_fwd.as<uint32_t>()};
+}
+R3QuotIn r3_quot_in(const cs_plonk_pk* pk, const PlonkWork& ws) {
+  return R3QuotIn{ws.ev[0].as<uint32_t>(), ws.ev[1].as<uint32_t>(), ws.ev[2].as<uint32_t>(), ws.ev[3].as<uint32_t>(),
+                  pk->dom4->tw_fwd.as<uint32_t>()};
+}
+R3KeyEvals key_evals(const cs_plonk_pk* pk, const PlonkWork& ws) {
+  const DevBuf *q = pk->q_evals, *s = pk->s_evals;
+  return R3KeyEvals{q[0].as<uint32_t>(), q[1].as<uint32_t>(), q[2].as<uint32_t>(), q[3].as<uint32_t>(),
+                    q[4].as<uint32_t>(), s[0].as<uint32_t>(), s[1].as<uint32_t>(), s[2].as<uint32_t>(),
+                    pk->lagrange.as<uint32_t>(), ws.buf[0].as<uint32_t>()};
+}
+
+// Round 3's tail (round3.rs:560-610): t and tz from 4n evaluations to coefficients, split into T1 T2 T3, committed into
+// three points at `out`
+template <class Cfg>
+int split_and_commit(cs_ctx* ctx, cs_plonk_pk* pk, PlonkWork& ws, const PlonkConsts& K, uint64_t* out) {
+  typedef typename Cfg::FrP FrP;
+  cudaStream_t st = ctx->stream;
+  const uint32_t n = pk->n, n4 = 4 * n;
+  const size_t pl = point_limbs64(pk->curve, CS_G1);
+  uint32_t *t = ws.t.as<uint32_t>(), *tz = ws.tz.as<uint32_t>();
+  uint32_t *t1 = ws.t1.as<uint32_t>(), *t2 = ws.t2.as<uint32_t>(), *t3 = ws.t3.as<uint32_t>();
+  CS_TRY(ntt_run(ctx, pk->dom4, t, 1, true, nullptr, st));
+  CS_TRY(ntt_run(ctx, pk->dom4, tz, 1, true, nullptr, st));
+  CS_LAUNCH(k_bit_reverse<FrP>, ceil_div(n4, 256), 256, 0, st, t, pk->log_n + 2, 1u);
+  CS_LAUNCH(k_bit_reverse<FrP>, ceil_div(n4, 256), 256, 0, st, tz, pk->log_n + 2, 1u);
+  CS_LAUNCH(k_plonk_tsplit<FrP>, ceil_div(n, 128), 128, 0, st, t, tz, n, K, t1, t2, t3);
+  Commit c[3] = {{t1, (size_t)n + 1, out}, {t2, (size_t)n + 1, out + pl}, {t3, (size_t)n + 6, out + 2 * pl}};
+  return commit_many<Cfg>(ctx, pk, c, 3);
+}
+
+// Round 4 (round4.rs:108-165): out = a b c at xi, z at xi w, s1 s2 at xi.  p: the coefficients of a b c z
+template <class Cfg>
+int evaluate(cs_ctx* ctx, const cs_plonk_pk* pk, const DevBuf* p, const host::HFp<typename Cfg::FrP>& xi, uint64_t* out) {
+  typedef host::HFp<typename Cfg::FrP> HR;
+  const size_t n = pk->n;
+  const HR xiw = xi * domain_gen<Cfg>(pk);
+  for (int k = 0; k < 3; k++) CS_TRY((eval_poly_t<Cfg>(ctx, p[k].as<uint64_t>(), n + 2, 1, xi.l, out + k * HR::N)));
+  CS_TRY((eval_poly_t<Cfg>(ctx, p[3].as<uint64_t>(), n + 3, 1, xiw.l, out + 3 * HR::N)));
+  CS_TRY((eval_poly_t<Cfg>(ctx, pk->s_coeffs[0].as<uint64_t>(), n, 1, xi.l, out + 4 * HR::N)));
+  return eval_poly_t<Cfg>(ctx, pk->s_coeffs[1].as<uint64_t>(), n, 1, xi.l, out + 5 * HR::N);
+}
+
+// Round 5 (round5.rs:284-340): Wxi = (linearisation numerator) / (X - xi) and Wxiw = (z - eval_zw) / (X - xi w),
+// committed into two points at `out`.  p: the coefficients of a b c z; pub: the public inputs after the leading slot;
+// ev: the opened a b c s1 s2 zw.  pub_terms = 0 leaves out the public polynomials, the constants and eval_zw, which
+// enter at one party only when the shares are additive (add_with_public on x_0).
+template <class Cfg>
+int opening_polys(cs_ctx* ctx, cs_plonk_pk* pk, PlonkWork& ws, const DevBuf* p, const uint64_t* pub, const PlonkConsts& K,
+                  const host::HFp<typename Cfg::FrP>& xi, const host::HFp<typename Cfg::FrP>& v,
+                  const host::HFp<typename Cfg::FrP>* ev, int pub_terms, uint64_t* out) {
+  typedef typename Cfg::FrP FrP;
+  const uint32_t n = pk->n;
+  const size_t pl = point_limbs64(pk->curve, CS_G1);
+  PlonkLinW W;
+  CS_TRY(lin_weights<Cfg>(pk, pub, K, xi, v, ev, W));
+  const DevBuf *q = pk->q_coeffs, *s = pk->s_coeffs;
+  const PlonkLinIn li{q[0].as<uint32_t>(),  q[1].as<uint32_t>(),  q[2].as<uint32_t>(),  q[3].as<uint32_t>(),
+                      q[4].as<uint32_t>(),  s[0].as<uint32_t>(),  s[1].as<uint32_t>(),  s[2].as<uint32_t>(),
+                      p[0].as<uint32_t>(),  p[1].as<uint32_t>(),  p[2].as<uint32_t>(),  p[3].as<uint32_t>(),
+                      ws.t1.as<uint32_t>(), ws.t2.as<uint32_t>(), ws.t3.as<uint32_t>()};
+  uint32_t *wxi = ws.tmp0.as<uint32_t>(), *wxiw = ws.tmp1.as<uint32_t>();
+  CS_LAUNCH(k_plonk_wxi_numerator<FrP>, ceil_div(n + 6, 128), 128, 0, ctx->stream, li, W, n, pub_terms, wxi);
+  CS_TRY(divide_by_linear<Cfg>(ctx, ws, wxi, n + 6, xi, nullptr));
+  CS_CUDA(cudaMemcpyAsync(wxiw, p[3].as<uint32_t>(), (size_t)(n + 3) * 32, cudaMemcpyDeviceToDevice, ctx->stream));
+  CS_TRY(divide_by_linear<Cfg>(ctx, ws, wxiw, n + 3, xi * domain_gen<Cfg>(pk), pub_terms ? &ev[5] : nullptr));
+  Commit c[2] = {{wxi, (size_t)n + 5, out}, {wxiw, (size_t)n + 2, out + pl}};
+  return commit_many<Cfg>(ctx, pk, c, 2);
+}
+
 template <class Cfg>
 int plonk_prove_plain_t(cs_ctx* ctx, cs_plonk_pk* pk, const uint64_t* h_pub, const uint64_t* h_wit, const uint64_t* h_blind,
                         uint64_t* out_points, uint64_t* out_evals) {
   typedef typename Cfg::FrP FrP;
   typedef host::HFp<FrP> HR;
   constexpr int NW = FrP::N;
-  const uint32_t n = pk->n, n4 = 4 * n, npub = pk->n_public;
+  PlonkWork& ws = pk->ws;
+  const uint32_t n = pk->n;
   const size_t pl = point_limbs64(pk->curve, CS_G1);
   cudaStream_t st = ctx->stream;
   CS_CUDA(cudaSetDevice(ctx->device));
   HR b[11];
   memcpy(b, h_blind, sizeof(b));
-  // ---- init round (round1.rs:191-252): w = 0 | public[1..] | witness | additions
-  uint32_t* w = pk->w.as<uint32_t>();
-  const uint32_t n_priv = pk->n_vars - pk->n_additions - npub - 1;
-  CS_CUDA(cudaMemsetAsync(w, 0, 32, st));  // types.rs:118-120: the leading one is replaced by zero
-  if (npub) CS_CUDA(cudaMemcpyAsync(w + NW, h_pub + HR::N, (size_t)npub * 32, cudaMemcpyHostToDevice, st));
-  if (n_priv) CS_CUDA(cudaMemcpyAsync(w + (size_t)(npub + 1) * NW, h_wit, (size_t)n_priv * 32, cudaMemcpyHostToDevice, st));
-  {
-    uint32_t lo = 0;
-    for (uint32_t hi : pk->level_ends) {
-      CS_LAUNCH(k_plonk_additions<FrP>, ceil_div(hi - lo, 128), 128, 0, st, pk->add_order.as<uint32_t>(), lo, hi,
-                pk->add_ids.as<uint32_t>(), pk->add_factors.as<uint32_t>(), pk->n_vars - pk->n_additions, 1u, w);
-      lo = hi;
-    }
-  }
-  // ---- round 1 (round1.rs:108-189, 255-320)
-  const uint32_t* maps[3] = {pk->map_a.as<uint32_t>(), pk->map_b.as<uint32_t>(), pk->map_c.as<uint32_t>()};
-  uint32_t *buf[3], *poly[4], *ev[4];
-  for (int i = 0; i < 3; i++) buf[i] = pk->buf[i].as<uint32_t>();
-  for (int i = 0; i < 4; i++) { poly[i] = pk->poly[i].as<uint32_t>(); ev[i] = pk->ev[i].as<uint32_t>(); }
-  for (int k = 0; k < 3; k++) {
-    CS_LAUNCH(k_plonk_gather<FrP>, ceil_div(n, 256), 256, 0, st, maps[k], pk->n_constraints, n, 1u, w, buf[k]);
-    CS_CUDA(cudaMemcpyAsync(poly[k], buf[k], (size_t)n * 32, cudaMemcpyDeviceToDevice, st));
-    CS_TRY(interpolate_and_extend<Cfg>(ctx, pk, poly[k], ev[k]));
-    CS_TRY(blind<Cfg>(ctx, poly[k], n, b + 2 * k, 2));
-  }
   uint64_t* P = out_points;  // A B C Z T1 T2 T3 Wxi Wxiw
-  {
-    Commit c[3] = {{poly[0], (size_t)n + 2, P}, {poly[1], (size_t)n + 2, P + pl}, {poly[2], (size_t)n + 2, P + 2 * pl}};
-    CS_TRY(commit_many<Cfg>(ctx, pk, c, 3));
-  }
+  // ---- init round, round 1
+  CS_TRY(load_witness<Cfg>(ctx, pk, ws, h_pub, h_wit, 1, 0));
+  for (int k = 0; k < 3; k++) CS_TRY(wire_poly<Cfg>(ctx, pk, ws, k, 1, b + 2 * k));
+  CS_TRY(commit_polys<Cfg>(ctx, pk, ws.poly, 3, (size_t)n + 2, P));
   // ---- round 2 (round2.rs:197-250)
-  HR k1, k2;
-  memcpy(k1.l, pk->k1.data(), sizeof(k1.l));
-  memcpy(k2.l, pk->k2.data(), sizeof(k2.l));
-  Transcript<Cfg> tr;
-  for (int i = 0; i < 8; i++) tr.add_point(pk->vk_points.data() + i * pl);
-  for (uint32_t i = 0; i < npub; i++) {
-    HR v;
-    memcpy(v.l, h_pub + (size_t)(i + 1) * HR::N, sizeof(v.l));
-    tr.add_scalar(v);
-  }
-  for (int i = 0; i < 3; i++) tr.add_point(P + i * pl);
-  const HR beta = tr.get_challenge();
-  tr = Transcript<Cfg>();
-  tr.add_scalar(beta);
-  const HR gamma = tr.get_challenge();
+  Challenges<Cfg> ch;
+  ch.round2(pk, h_pub, P);
   PlonkConsts K;
-  memset(&K, 0, sizeof(K));
-  for (int i = 0; i < 11; i++) put(K.b[i], b[i]);
-  put(K.beta, beta); put(K.gamma, gamma); put(K.k1, k1); put(K.k2, k2);
-  uint32_t *num = pk->t.as<uint32_t>(), *den = num + (size_t)n * NW, *sden = den + (size_t)n * NW;  // scratch inside t (4n)
-  const uint32_t* tw4 = pk->dom4->tw_fwd.template as<uint32_t>();
-  CS_LAUNCH(k_plonk_numden<FrP>, ceil_div(n, 128), 128, 0, st, buf[0], buf[1], buf[2], pk->s_evals[0].as<uint32_t>(),
-            pk->s_evals[1].as<uint32_t>(), pk->s_evals[2].as<uint32_t>(), tw4, n, K, num, den);
-  CS_TRY((scan<FrP, 0>(ctx, pk, num, num, n, 0)));    // running products of the numerators (in place)
-  CS_TRY((scan<FrP, 0>(ctx, pk, den, sden, n, 1)));   // suffix products of the denominators
+  init_consts<Cfg>(K, pk, b, 1);
+  put(K.beta, ch.beta);
+  put(K.gamma, ch.gamma);
+  uint32_t *num = ws.t.as<uint32_t>(), *den = num + (size_t)n * NW, *sden = den + (size_t)n * NW;  // scratch inside t (4n)
+  const R3Round2In in = r3_round2_in(pk, ws);
+  CS_LAUNCH(k_plonk_numden<FrP>, ceil_div(n, 128), 128, 0, st, in.a, in.b, in.c, in.s1, in.s2, in.s3, in.tw4, n, K, num, den);
+  CS_TRY((scan<FrP, 0>(ctx, ws, num, num, n, 0)));    // running products of the numerators (in place)
+  CS_TRY((scan<FrP, 0>(ctx, ws, den, sden, n, 1)));   // suffix products of the denominators
   HR total;
   CS_CUDA(cudaMemcpyAsync(total.l, sden, sizeof(total.l), cudaMemcpyDeviceToHost, st));
   CS_CUDA(cudaStreamSynchronize(st));
   if (total.is_zero()) return fail(CS_ERR_ARG, "Cannot invert zero");  // mpc/plain.rs:206-208
   HR inv_total = total.inverse();
-  uint32_t* d_small = pk->small.as<uint32_t>();
+  uint32_t* d_small = ws.small.as<uint32_t>();
   CS_CUDA(cudaMemcpyAsync(d_small, inv_total.l, sizeof(inv_total.l), cudaMemcpyHostToDevice, st));
-  CS_LAUNCH(k_plonk_zbuf<FrP>, ceil_div(n, 128), 128, 0, st, num, sden, d_small, n, poly[3]);
+  CS_LAUNCH(k_plonk_zbuf<FrP>, ceil_div(n, 128), 128, 0, st, num, sden, d_small, n, ws.poly[3].as<uint32_t>());
   CS_CUDA(cudaStreamSynchronize(st));  // inv_total is a stack variable
-  CS_TRY(interpolate_and_extend<Cfg>(ctx, pk, poly[3], ev[3]));
-  CS_TRY(blind<Cfg>(ctx, poly[3], n, b + 6, 3));
-  {
-    Commit c[1] = {{poly[3], (size_t)n + 3, P + 3 * pl}};
-    CS_TRY(commit_many<Cfg>(ctx, pk, c, 1));
-  }
+  CS_TRY(z_poly<Cfg>(ctx, pk, ws, 1, b + 6));
+  CS_TRY(commit_polys<Cfg>(ctx, pk, ws.poly + 3, 1, (size_t)n + 3, P + 3 * pl));
   // ---- round 3 (round3.rs:560-610)
-  tr = Transcript<Cfg>();
-  tr.add_scalar(beta);
-  tr.add_scalar(gamma);
-  tr.add_point(P + 3 * pl);
-  const HR alpha = tr.get_challenge();
-  const HR alpha2 = alpha.sqr();
-  put(K.alpha, alpha); put(K.alpha2, alpha2);
-  CS_TRY(quotient_consts<Cfg>(pk->curve, K));
-  PlonkQuotIn qi;
-  qi.a = ev[0]; qi.b = ev[1]; qi.c = ev[2]; qi.z = ev[3];
-  qi.qm = pk->q_evals[0].as<uint32_t>(); qi.ql = pk->q_evals[1].as<uint32_t>(); qi.qr = pk->q_evals[2].as<uint32_t>();
-  qi.qo = pk->q_evals[3].as<uint32_t>(); qi.qc = pk->q_evals[4].as<uint32_t>();
-  qi.s1 = pk->s_evals[0].as<uint32_t>(); qi.s2 = pk->s_evals[1].as<uint32_t>(); qi.s3 = pk->s_evals[2].as<uint32_t>();
-  qi.lagrange = pk->lagrange.as<uint32_t>(); qi.buf_a = buf[0]; qi.tw4 = tw4;
-  uint32_t *t = pk->t.as<uint32_t>(), *tz = pk->tz.as<uint32_t>();
-  CS_LAUNCH(k_plonk_quotient<FrP>, ceil_div(n4, 128), 128, 0, st, qi, n, pk->nlag, K, t, tz);
-  CS_TRY(ntt_run(ctx, pk->dom4, t, 1, true, nullptr, st));
-  CS_TRY(ntt_run(ctx, pk->dom4, tz, 1, true, nullptr, st));
-  CS_LAUNCH(k_bit_reverse<FrP>, ceil_div(n4, 256), 256, 0, st, t, pk->log_n + 2, 1u);
-  CS_LAUNCH(k_bit_reverse<FrP>, ceil_div(n4, 256), 256, 0, st, tz, pk->log_n + 2, 1u);
-  uint32_t *t1 = pk->t1.as<uint32_t>(), *t2 = pk->t2.as<uint32_t>(), *t3 = pk->t3.as<uint32_t>();
-  CS_LAUNCH(k_plonk_tsplit<FrP>, ceil_div(n, 128), 128, 0, st, t, tz, n, K, t1, t2, t3);
-  {
-    Commit c[3] = {{t1, (size_t)n + 1, P + 4 * pl}, {t2, (size_t)n + 1, P + 5 * pl}, {t3, (size_t)n + 6, P + 6 * pl}};
-    CS_TRY(commit_many<Cfg>(ctx, pk, c, 3));
-  }
-  // ---- round 4 (round4.rs:108-165)
-  tr = Transcript<Cfg>();
-  tr.add_scalar(alpha);
-  for (int i = 4; i < 7; i++) tr.add_point(P + i * pl);
-  const HR xi = tr.get_challenge();
-  HR w_n;
-  memcpy(w_n.l, pk->dom->group_gen.data(), sizeof(w_n.l));
-  const HR xiw = xi * w_n;
-  HR ea, eb, ec, ezw, es1, es2;
-  CS_TRY((eval_poly_t<Cfg>(ctx, reinterpret_cast<uint64_t*>(poly[0]), (size_t)n + 2, 1, xi.l, ea.l)));
-  CS_TRY((eval_poly_t<Cfg>(ctx, reinterpret_cast<uint64_t*>(poly[1]), (size_t)n + 2, 1, xi.l, eb.l)));
-  CS_TRY((eval_poly_t<Cfg>(ctx, reinterpret_cast<uint64_t*>(poly[2]), (size_t)n + 2, 1, xi.l, ec.l)));
-  CS_TRY((eval_poly_t<Cfg>(ctx, reinterpret_cast<uint64_t*>(poly[3]), (size_t)n + 3, 1, xiw.l, ezw.l)));
-  CS_TRY((eval_poly_t<Cfg>(ctx, pk->s_coeffs[0].as<uint64_t>(), (size_t)n, 1, xi.l, es1.l)));
-  CS_TRY((eval_poly_t<Cfg>(ctx, pk->s_coeffs[1].as<uint64_t>(), (size_t)n, 1, xi.l, es2.l)));
-  // ---- round 5 (round5.rs:284-340)
-  tr = Transcript<Cfg>();
-  tr.add_scalar(xi); tr.add_scalar(ea); tr.add_scalar(eb); tr.add_scalar(ec);
-  tr.add_scalar(es1); tr.add_scalar(es2); tr.add_scalar(ezw);
-  const HR evs5[6] = {ea, eb, ec, es1, es2, ezw};
-  PlonkLinW W;
-  CS_TRY(lin_weights<Cfg>(pk, h_pub + HR::N, K, xi, tr.get_challenge(), evs5, W));
-  PlonkLinIn li;
-  li.qm = pk->q_coeffs[0].as<uint32_t>(); li.ql = pk->q_coeffs[1].as<uint32_t>(); li.qr = pk->q_coeffs[2].as<uint32_t>();
-  li.qo = pk->q_coeffs[3].as<uint32_t>(); li.qc = pk->q_coeffs[4].as<uint32_t>();
-  li.s1 = pk->s_coeffs[0].as<uint32_t>(); li.s2 = pk->s_coeffs[1].as<uint32_t>(); li.s3 = pk->s_coeffs[2].as<uint32_t>();
-  li.pa = poly[0]; li.pb = poly[1]; li.pc = poly[2]; li.pz = poly[3]; li.t1 = t1; li.t2 = t2; li.t3 = t3;
-  uint32_t *wxi = pk->tmp0.as<uint32_t>(), *wxiw = pk->tmp1.as<uint32_t>();
-  CS_LAUNCH(k_plonk_wxi_numerator<FrP>, ceil_div(n + 6, 128), 128, 0, st, li, W, n, 1, wxi);
-  CS_TRY(divide_by_linear<Cfg>(ctx, pk, wxi, n + 6, xi, nullptr));
-  CS_CUDA(cudaMemcpyAsync(wxiw, poly[3], (size_t)(n + 3) * 32, cudaMemcpyDeviceToDevice, st));
-  CS_TRY(divide_by_linear<Cfg>(ctx, pk, wxiw, n + 3, xiw, &ezw));
-  {
-    Commit c[2] = {{wxi, (size_t)n + 5, P + 7 * pl}, {wxiw, (size_t)n + 2, P + 8 * pl}};
-    CS_TRY(commit_many<Cfg>(ctx, pk, c, 2));
-  }
-  HR evs[6] = {ea, eb, ec, es1, es2, ezw};
-  memcpy(out_evals, evs, sizeof(evs));
+  ch.round3(P + 3 * pl);
+  CS_TRY(set_alpha<Cfg>(pk, K, ch.alpha));
+  const R3QuotIn q = r3_quot_in(pk, ws);
+  const R3KeyEvals E = key_evals(pk, ws);
+  const PlonkQuotIn qi{q.a, q.b, q.c, q.z, E.qm, E.ql, E.qr, E.qo, E.qc, E.s1, E.s2, E.s3, E.lagrange, E.buf_a, q.tw4};
+  CS_LAUNCH(k_plonk_quotient<FrP>, ceil_div(4 * n, 128), 128, 0, st, qi, n, pk->nlag, K, ws.t.as<uint32_t>(), ws.tz.as<uint32_t>());
+  CS_TRY(split_and_commit<Cfg>(ctx, pk, ws, K, P + 4 * pl));
+  // ---- round 4
+  ch.round4(P + 4 * pl);
+  HR e[6];  // a b c zw s1 s2
+  CS_TRY(evaluate<Cfg>(ctx, pk, ws.poly, ch.xi, e[0].l));
+  // ---- round 5
+  const HR ev[6] = {e[0], e[1], e[2], e[4], e[5], e[3]};  // the proof's order: a b c s1 s2 zw
+  ch.round5(ev);
+  CS_TRY(opening_polys<Cfg>(ctx, pk, ws, ws.poly, h_pub + HR::N, K, ch.xi, ch.v, ev, 1, P + 7 * pl));
+  memcpy(out_evals, ev, sizeof(ev));
   return 0;
 }
 
@@ -525,7 +661,9 @@ struct cs_plonk_rep3 {
   cs_ctx* ctx = nullptr;
   cs_plonk_pk* pk = nullptr;
   int party = 0;
-  DevBuf w, buf[3], polysh[4], ev[4], polyadd[4], arena, addv, pubv, t, tz, t1, t2, t3, tmp0, tmp1, totals, small;
+  PlonkWork ws;       // w, buf, poly and ev hold share pairs
+  DevBuf polyadd[4];  // component 0 of a b c z: this party's additive share, what it commits and evaluates
+  DevBuf arena, addv, pubv;
   uint32_t* next_arena = nullptr;
   const uint32_t* peer_out[2] = {nullptr, nullptr};  // previous / next party's additive-out vector (cs_plonk_rep3_connect_io)
   size_t slot_words = 0;  // 32-bit words per arena slot (4n shares)
@@ -541,30 +679,15 @@ namespace {
 
 constexpr int R3_SLOTS = 12;
 
-template <class Cfg>
-int r3_create_t(cs_plonk_rep3* s) {
-  const cs_plonk_pk* pk = s->pk;
-  const size_t n = pk->n;
-  CS_TRY(s->w.reserve((size_t)pk->n_vars * 64));
-  for (int i = 0; i < 3; i++) CS_TRY(s->buf[i].reserve(n * 64));
-  for (int i = 0; i < 4; i++) {
-    CS_TRY(s->polysh[i].reserve((n + 8) * 64));
-    CS_TRY(s->polyadd[i].reserve((n + 8) * 32));
-    CS_TRY(s->ev[i].reserve(4 * n * 64));
-  }
+int r3_create(cs_plonk_rep3* s) {
+  const size_t n = s->pk->n;
+  CS_TRY(s->ws.reserve(n, s->pk->n_vars, 2));
+  for (DevBuf& p : s->polyadd) CS_TRY(p.reserve((n + 8) * 32));
   s->slot_words = 4 * n * 2 * 8;
   CS_TRY(s->arena.reserve((size_t)R3_SLOTS * s->slot_words * 4));
   CS_CUDA(cudaMemsetAsync(s->arena.p, 0, (size_t)R3_SLOTS * s->slot_words * 4, s->ctx->stream));
   CS_TRY(s->addv.reserve((2 * n + 2) * 32));
   CS_TRY(s->pubv.reserve((8 * n + 16) * 32));  // 1/G | 1/Q | scan scratch (2n + 2) | opened vectors (2n + 1)
-  CS_TRY(s->t.reserve(4 * n * 32));
-  CS_TRY(s->tz.reserve(4 * n * 32));
-  CS_TRY(s->t1.reserve((n + 8) * 32));
-  CS_TRY(s->t2.reserve((n + 8) * 32));
-  CS_TRY(s->t3.reserve((n + 8) * 32));
-  CS_TRY(s->tmp0.reserve((n + 8) * 32));
-  CS_TRY(s->tmp1.reserve((n + 8) * 32));
-  CS_TRY(s->small.reserve(8192));
   CS_CUDA(cudaStreamSynchronize(s->ctx->stream));
   return 0;
 }
@@ -573,80 +696,41 @@ inline uint32_t* r3_slot(cs_plonk_rep3* s, int k) { return s->arena.as<uint32_t>
 inline uint32_t* r3_peer(cs_plonk_rep3* s, int k) { return s->next_arena ? s->next_arena + (size_t)k * s->slot_words : nullptr; }
 
 template <class Cfg>
-R3Round2In r3_round2_in(cs_plonk_rep3* s) {
-  R3Round2In in;
-  in.a = s->buf[0].as<uint32_t>(); in.b = s->buf[1].as<uint32_t>(); in.c = s->buf[2].as<uint32_t>();
-  in.s1 = s->pk->s_evals[0].as<uint32_t>(); in.s2 = s->pk->s_evals[1].as<uint32_t>(); in.s3 = s->pk->s_evals[2].as<uint32_t>();
-  in.tw4 = s->pk->dom4->tw_fwd.template as<uint32_t>();
-  return in;
-}
-
-template <class Cfg>
 int r3_round1_t(cs_plonk_rep3* s, const uint64_t* h_pub, const uint64_t* h_wit_shares, const uint64_t* h_blind, uint64_t* out_points) {
   typedef typename Cfg::FrP FrP;
   typedef host::HFp<FrP> HR;
-  constexpr int NW = FrP::N;
   cs_ctx* ctx = s->ctx;
   cs_plonk_pk* pk = s->pk;
-  cudaStream_t st = ctx->stream;
-  const uint32_t n = pk->n, npub = pk->n_public;
-  const uint32_t n_priv = pk->n_vars - pk->n_additions - npub - 1;
-  // w = 0 | promote(public) | witness shares | additions   (promote_to_trivial_share, rep3/arithmetic.rs:41-50)
-  std::vector<uint64_t> stage((size_t)(npub + 1) * 2 * HR::N, 0);
-  for (uint32_t j = 1; j <= npub; j++)
-    if (s->party < 2) memcpy(&stage[((size_t)j * 2 + s->party) * HR::N], h_pub + (size_t)j * HR::N, sizeof(HR));
-  s->pub.assign(h_pub + HR::N, h_pub + (size_t)(npub + 1) * HR::N);
-  uint32_t* w = s->w.as<uint32_t>();
-  CS_CUDA(cudaMemcpyAsync(w, stage.data(), stage.size() * 8, cudaMemcpyHostToDevice, st));
-  if (n_priv) CS_CUDA(cudaMemcpyAsync(w + (size_t)(npub + 1) * 2 * NW, h_wit_shares, (size_t)n_priv * 64, cudaMemcpyHostToDevice, st));
-  CS_CUDA(cudaStreamSynchronize(st));  // `stage` is a local vector
-  uint32_t lo = 0;
-  for (uint32_t hi : pk->level_ends) {
-    CS_LAUNCH(k_plonk_additions<FrP>, ceil_div(hi - lo, 128), 128, 0, st, pk->add_order.as<uint32_t>(), lo, hi,
-              pk->add_ids.as<uint32_t>(), pk->add_factors.as<uint32_t>(), pk->n_vars - pk->n_additions, 2u, w);
-    lo = hi;
-  }
+  const uint32_t n = pk->n;
+  s->pub.assign(h_pub + HR::N, h_pub + (size_t)(pk->n_public + 1) * HR::N);
+  CS_TRY(load_witness<Cfg>(ctx, pk, s->ws, h_pub, h_wit_shares, 2, s->party < 2 ? s->party : -1));
   HR bsh[22];
   memcpy(bsh, h_blind, sizeof(bsh));
-  memset(&s->K, 0, sizeof(s->K));
+  init_consts<Cfg>(s->K, pk, bsh, 2);
   memset(&s->B, 0, sizeof(s->B));
-  for (int i = 0; i < 11; i++) put(s->K.b[i], bsh[2 * i]);  // additive part of each blinder
   for (int i = 0; i < 9; i++) { put(s->B.b[i].v[0], bsh[2 * i]); put(s->B.b[i].v[1], bsh[2 * i + 1]); }
-  put(s->K.k1, *reinterpret_cast<const HR*>(pk->k1.data()));
-  put(s->K.k2, *reinterpret_cast<const HR*>(pk->k2.data()));
-  const uint32_t* maps[3] = {pk->map_a.as<uint32_t>(), pk->map_b.as<uint32_t>(), pk->map_c.as<uint32_t>()};
-  const size_t pl = point_limbs64(pk->curve, CS_G1);
-  Commit c[3];
   for (int k = 0; k < 3; k++) {
-    uint32_t* buf = s->buf[k].as<uint32_t>();
-    uint32_t* ps = s->polysh[k].as<uint32_t>();
-    CS_LAUNCH(k_plonk_gather<FrP>, ceil_div(n, 256), 256, 0, st, maps[k], pk->n_constraints, n, 2u, w, buf);
-    CS_CUDA(cudaMemcpyAsync(ps, buf, (size_t)n * 64, cudaMemcpyDeviceToDevice, st));
-    CS_TRY(interpolate_and_extend<Cfg>(ctx, pk, ps, s->ev[k].as<uint32_t>(), 2));
-    CS_TRY(blind<Cfg>(ctx, ps, n, bsh + 4 * k, 2, 2));
-    CS_LAUNCH(k_extract_component<FrP>, ceil_div(n + 2, 256), 256, 0, st, ps, n + 2, 2u, 0u, s->polyadd[k].as<uint32_t>());
-    c[k] = Commit{s->polyadd[k].as<uint32_t>(), (size_t)n + 2, out_points + k * pl};
+    CS_TRY(wire_poly<Cfg>(ctx, pk, s->ws, k, 2, bsh + 4 * k));
+    CS_LAUNCH(k_extract_component<FrP>, ceil_div(n + 2, 256), 256, 0, ctx->stream, s->ws.poly[k].as<uint32_t>(), n + 2, 2u, 0u,
+              s->polyadd[k].as<uint32_t>());
   }
-  CS_TRY(commit_many<Cfg>(ctx, pk, c, 3));
-  return 0;
+  return commit_polys<Cfg>(ctx, pk, s->polyadd, 3, (size_t)n + 2, out_points);
 }
 
 // elementwise inverse of `cnt` public values at `v` (device) into `out`; scratch: 2 cnt elements at `scr`
-// H: a session with `ctx`, `totals` and `small` (Rep3 or Shamir)
-template <class Cfg, class H>
-int r3_batch_inverse(H* s, const uint32_t* v, uint32_t cnt, uint32_t* scr, uint32_t* out) {
+template <class Cfg>
+int r3_batch_inverse(cs_ctx* ctx, PlonkWork& ws, const uint32_t* v, uint32_t cnt, uint32_t* scr, uint32_t* out) {
   typedef typename Cfg::FrP FrP;
   typedef host::HFp<FrP> HR;
-  cs_ctx* ctx = s->ctx;
   uint32_t *pre = scr, *suf = scr + (size_t)cnt * FrP::N;
-  CS_TRY((scan<FrP, 0>(ctx, s, v, pre, cnt, 0)));
-  CS_TRY((scan<FrP, 0>(ctx, s, v, suf, cnt, 1)));
+  CS_TRY((scan<FrP, 0>(ctx, ws, v, pre, cnt, 0)));
+  CS_TRY((scan<FrP, 0>(ctx, ws, v, suf, cnt, 1)));
   HR total;
   CS_CUDA(cudaMemcpyAsync(total.l, suf, sizeof(total.l), cudaMemcpyDeviceToHost, ctx->stream));
   CS_CUDA(cudaStreamSynchronize(ctx->stream));
   if (total.is_zero()) return fail(CS_ERR_ARG, "Cannot invert zero");  // rep3 inv_vec, arithmetic.rs:245-262
   HR it = total.inverse();
-  uint32_t* d_it = s->small.template as<uint32_t>() + 128 * FrP::N;
+  uint32_t* d_it = ws.small.as<uint32_t>() + 128 * FrP::N;
   CS_CUDA(cudaMemcpyAsync(d_it, it.l, sizeof(it.l), cudaMemcpyHostToDevice, ctx->stream));
   CS_LAUNCH(k_batch_inverse<FrP>, ceil_div(cnt, 128), 128, 0, ctx->stream, pre, suf, d_it, cnt, out);
   CS_CUDA(cudaStreamSynchronize(ctx->stream));  // `it` is a stack variable
@@ -660,9 +744,9 @@ int r3_step_t(cs_plonk_rep3* s, int step, const uint64_t* h_in, uint64_t* h_out)
   constexpr int NW = FrP::N;
   cs_ctx* ctx = s->ctx;
   cs_plonk_pk* pk = s->pk;
+  PlonkWork& ws = s->ws;
   cudaStream_t st = ctx->stream;
   const uint32_t n = pk->n, n4 = 4 * n;
-  const size_t pl = point_limbs64(pk->curve, CS_G1);
   const unsigned gb = ceil_div(n, 128);
   uint32_t *addv = s->addv.as<uint32_t>(), *pubv = s->pubv.as<uint32_t>();
   // public vectors: [0, n) 1/G | [n, 2n+1) 1/Q | then scratch
@@ -671,13 +755,13 @@ int r3_step_t(cs_plonk_rep3* s, int step, const uint64_t* h_in, uint64_t* h_out)
     case CS_PLONK_R3_ROUND2_A: {  // in: beta, gamma
       memcpy(s->K.beta, h_in, 32);
       memcpy(s->K.gamma, h_in + HR::N, 32);
-      CS_LAUNCH(k_r3_round2_a<Rep3Pol<FrP>>, gb, 128, 0, st, r3_round2_in<Cfg>(s), s->K, n, s->party, s->prf, s->ctr, r3_slot(s, 0),
+      CS_LAUNCH(k_r3_round2_a<Rep3Pol<FrP>>, gb, 128, 0, st, r3_round2_in(pk, ws), s->K, n, s->party, s->prf, s->ctr, r3_slot(s, 0),
                 r3_slot(s, 1), r3_peer(s, 0), r3_peer(s, 1));
       s->ctr += 2 * (uint64_t)n;
       break;
     }
     case CS_PLONK_R3_ROUND2_B: {
-      CS_LAUNCH(k_r3_round2_b<Rep3Pol<FrP>>, gb, 128, 0, st, r3_round2_in<Cfg>(s), s->K, n, s->party, s->prf, s->ctr, r3_slot(s, 0),
+      CS_LAUNCH(k_r3_round2_b<Rep3Pol<FrP>>, gb, 128, 0, st, r3_round2_in(pk, ws), s->K, n, s->party, s->prf, s->ctr, r3_slot(s, 0),
                 r3_slot(s, 1), r3_slot(s, 2), r3_slot(s, 3), r3_peer(s, 2), r3_peer(s, 3));
       s->ctr += 2 * (uint64_t)n;
       break;
@@ -695,8 +779,8 @@ int r3_step_t(cs_plonk_rep3* s, int step, const uint64_t* h_in, uint64_t* h_out)
     case CS_PLONK_R3_ROUND2_D: {  // in: opened G (n) | Q (n + 1)
       uint32_t* opened = pscr + (size_t)(4 * n + 4) * NW;  // h_in == NULL: the driver summed the parties' vectors in place
       if (h_in) CS_CUDA(cudaMemcpyAsync(opened, h_in, (size_t)(2 * n + 1) * 32, cudaMemcpyHostToDevice, st));
-      CS_TRY(r3_batch_inverse<Cfg>(s, opened, n, pscr, ginv));
-      CS_TRY(r3_batch_inverse<Cfg>(s, opened + (size_t)n * NW, n + 1, pscr, qinv));
+      CS_TRY(r3_batch_inverse<Cfg>(ctx, ws, opened, n, pscr, ginv));
+      CS_TRY(r3_batch_inverse<Cfg>(ctx, ws, opened + (size_t)n * NW, n + 1, pscr, qinv));
       CS_LAUNCH(k_r3_round2_d<Rep3Pol<FrP>>, gb, 128, 0, st, r3_slot(s, 2), ginv, qinv, n, s->prf, s->rbase, s->ctr, r3_slot(s, 4),
                 r3_slot(s, 5), r3_peer(s, 4), r3_peer(s, 5));
       s->ctr += 2 * (uint64_t)n;
@@ -718,88 +802,40 @@ int r3_step_t(cs_plonk_rep3* s, int step, const uint64_t* h_in, uint64_t* h_out)
       uint32_t* y = pscr;
       if (h_in) CS_CUDA(cudaMemcpyAsync(y, h_in, (size_t)n * 32, cudaMemcpyHostToDevice, st));
       else CS_CUDA(cudaMemcpyAsync(y, pscr + (size_t)(4 * n + 4) * NW, (size_t)n * 32, cudaMemcpyDeviceToDevice, st));
-      CS_TRY((scan<FrP, 0>(ctx, s, y, y, n, 0)));
-      uint32_t* ps = s->polysh[3].as<uint32_t>();
-      CS_LAUNCH(k_r3_round2_g<Rep3Pol<FrP>>, gb, 128, 0, st, y, r3_slot(s, 5), n, ps);
-      CS_TRY(interpolate_and_extend<Cfg>(ctx, pk, ps, s->ev[3].as<uint32_t>(), 2));
+      CS_TRY((scan<FrP, 0>(ctx, ws, y, y, n, 0)));
+      CS_LAUNCH(k_r3_round2_g<Rep3Pol<FrP>>, gb, 128, 0, st, y, r3_slot(s, 5), n, ws.poly[3].as<uint32_t>());
       HR bsh[6];
       for (int i = 0; i < 3; i++) { memcpy(bsh[2 * i].l, s->B.b[6 + i].v[0], 32); memcpy(bsh[2 * i + 1].l, s->B.b[6 + i].v[1], 32); }
-      CS_TRY(blind<Cfg>(ctx, ps, n, bsh, 3, 2));
-      CS_LAUNCH(k_extract_component<FrP>, ceil_div(n + 3, 256), 256, 0, st, ps, n + 3, 2u, 0u, s->polyadd[3].as<uint32_t>());
-      Commit c[1] = {{s->polyadd[3].as<uint32_t>(), (size_t)n + 3, h_out}};
-      return commit_many<Cfg>(ctx, pk, c, 1);
+      CS_TRY(z_poly<Cfg>(ctx, pk, ws, 2, bsh));
+      CS_LAUNCH(k_extract_component<FrP>, ceil_div(n + 3, 256), 256, 0, st, ws.poly[3].as<uint32_t>(), n + 3, 2u, 0u,
+                s->polyadd[3].as<uint32_t>());
+      return commit_polys<Cfg>(ctx, pk, s->polyadd + 3, 1, (size_t)n + 3, h_out);
     }
     case CS_PLONK_R3_ROUND3_A: {  // in: alpha
       HR alpha;
       memcpy(alpha.l, h_in, 32);
-      put(s->K.alpha, alpha);
-      put(s->K.alpha2, alpha.sqr());
-      CS_TRY(quotient_consts<Cfg>(pk->curve, s->K));
-      R3QuotIn qi;
-      qi.a = s->ev[0].as<uint32_t>(); qi.b = s->ev[1].as<uint32_t>(); qi.c = s->ev[2].as<uint32_t>(); qi.z = s->ev[3].as<uint32_t>();
-      qi.tw4 = pk->dom4->tw_fwd.template as<uint32_t>();
-      CS_LAUNCH(k_r3_quot_l1<Rep3Pol<FrP>>, ceil_div(n4, 64), 64, 0, st, qi, s->B, n, s->prf, s->ctr, s->arena.as<uint32_t>(), s->next_arena,
-                s->slot_words);
+      CS_TRY(set_alpha<Cfg>(pk, s->K, alpha));
+      CS_LAUNCH(k_r3_quot_l1<Rep3Pol<FrP>>, ceil_div(n4, 64), 64, 0, st, r3_quot_in(pk, ws), s->B, n, s->prf, s->ctr,
+                s->arena.as<uint32_t>(), s->next_arena, s->slot_words);
       s->ctr += 12 * (uint64_t)n4;
       break;
     }
     case CS_PLONK_R3_ROUND3_B: {  // out: partial [t1] [t2] [t3]
-      R3QuotIn qi;
-      qi.a = s->ev[0].as<uint32_t>(); qi.b = s->ev[1].as<uint32_t>(); qi.c = s->ev[2].as<uint32_t>(); qi.z = s->ev[3].as<uint32_t>();
-      qi.tw4 = pk->dom4->tw_fwd.template as<uint32_t>();
-      R3KeyEvals E;
-      E.qm = pk->q_evals[0].as<uint32_t>(); E.ql = pk->q_evals[1].as<uint32_t>(); E.qr = pk->q_evals[2].as<uint32_t>();
-      E.qo = pk->q_evals[3].as<uint32_t>(); E.qc = pk->q_evals[4].as<uint32_t>();
-      E.s1 = pk->s_evals[0].as<uint32_t>(); E.s2 = pk->s_evals[1].as<uint32_t>(); E.s3 = pk->s_evals[2].as<uint32_t>();
-      E.lagrange = pk->lagrange.as<uint32_t>(); E.buf_a = s->buf[0].as<uint32_t>();
-      uint32_t *t = s->t.as<uint32_t>(), *tz = s->tz.as<uint32_t>();
-      CS_LAUNCH(k_r3_quot_l2<Rep3Pol<FrP>>, ceil_div(n4, 64), 64, 0, st, qi, s->B, E, n, pk->nlag, s->K, s->party, s->prf, s->ctr,
-                s->arena.as<uint32_t>(), s->slot_words, t, tz);
+      CS_LAUNCH(k_r3_quot_l2<Rep3Pol<FrP>>, ceil_div(n4, 64), 64, 0, st, r3_quot_in(pk, ws), s->B, key_evals(pk, ws), n, pk->nlag,
+                s->K, s->party, s->prf, s->ctr, s->arena.as<uint32_t>(), s->slot_words, ws.t.as<uint32_t>(), ws.tz.as<uint32_t>());
       s->ctr += 2 * (uint64_t)n4;
-      CS_TRY(ntt_run(ctx, pk->dom4, t, 1, true, nullptr, st));
-      CS_TRY(ntt_run(ctx, pk->dom4, tz, 1, true, nullptr, st));
-      CS_LAUNCH(k_bit_reverse<FrP>, ceil_div(n4, 256), 256, 0, st, t, pk->log_n + 2, 1u);
-      CS_LAUNCH(k_bit_reverse<FrP>, ceil_div(n4, 256), 256, 0, st, tz, pk->log_n + 2, 1u);
-      uint32_t *t1 = s->t1.as<uint32_t>(), *t2 = s->t2.as<uint32_t>(), *t3 = s->t3.as<uint32_t>();
-      CS_LAUNCH(k_plonk_tsplit<FrP>, gb, 128, 0, st, t, tz, n, s->K, t1, t2, t3);
-      Commit c[3] = {{t1, (size_t)n + 1, h_out}, {t2, (size_t)n + 1, h_out + pl}, {t3, (size_t)n + 6, h_out + 2 * pl}};
-      return commit_many<Cfg>(ctx, pk, c, 3);
+      return split_and_commit<Cfg>(ctx, pk, ws, s->K, h_out);
     }
     case CS_PLONK_R3_ROUND4: {  // in: xi; out: partial eval_a eval_b eval_c eval_zw, then public eval_s1 eval_s2
-      HR xi, w_n;
+      HR xi;
       memcpy(xi.l, h_in, 32);
-      memcpy(w_n.l, pk->dom->group_gen.data(), sizeof(w_n.l));
-      HR xiw = xi * w_n;
-      for (int k = 0; k < 3; k++)
-        CS_TRY((eval_poly_t<Cfg>(ctx, s->polyadd[k].as<uint64_t>(), (size_t)n + 2, 1, xi.l, h_out + (size_t)k * HR::N)));
-      CS_TRY((eval_poly_t<Cfg>(ctx, s->polyadd[3].as<uint64_t>(), (size_t)n + 3, 1, xiw.l, h_out + 3 * HR::N)));
-      CS_TRY((eval_poly_t<Cfg>(ctx, pk->s_coeffs[0].as<uint64_t>(), (size_t)n, 1, xi.l, h_out + 4 * HR::N)));
-      CS_TRY((eval_poly_t<Cfg>(ctx, pk->s_coeffs[1].as<uint64_t>(), (size_t)n, 1, xi.l, h_out + 5 * HR::N)));
-      return 0;
+      return evaluate<Cfg>(ctx, pk, s->polyadd, xi, h_out);
     }
     case CS_PLONK_R3_ROUND5: {  // in: xi, v0, eval_a eval_b eval_c eval_s1 eval_s2 eval_zw (opened); out: partial [Wxi] [Wxiw]
       HR in[8];
       memcpy(in, h_in, sizeof(in));
-      const HR xi = in[0], ezw = in[7];
-      HR w_n;
-      memcpy(w_n.l, pk->dom->group_gen.data(), sizeof(w_n.l));
-      const HR xiw = xi * w_n;
-      PlonkLinW W;
-      CS_TRY(lin_weights<Cfg>(pk, s->pub.data(), s->K, xi, in[1], in + 2, W));
-      PlonkLinIn li;
-      li.qm = pk->q_coeffs[0].as<uint32_t>(); li.ql = pk->q_coeffs[1].as<uint32_t>(); li.qr = pk->q_coeffs[2].as<uint32_t>();
-      li.qo = pk->q_coeffs[3].as<uint32_t>(); li.qc = pk->q_coeffs[4].as<uint32_t>();
-      li.s1 = pk->s_coeffs[0].as<uint32_t>(); li.s2 = pk->s_coeffs[1].as<uint32_t>(); li.s3 = pk->s_coeffs[2].as<uint32_t>();
-      li.pa = s->polyadd[0].as<uint32_t>(); li.pb = s->polyadd[1].as<uint32_t>(); li.pc = s->polyadd[2].as<uint32_t>();
-      li.pz = s->polyadd[3].as<uint32_t>(); li.t1 = s->t1.as<uint32_t>(); li.t2 = s->t2.as<uint32_t>(); li.t3 = s->t3.as<uint32_t>();
-      const int pub = s->party == 0;  // public polynomials and constants enter once (add_with_public on x_0)
-      uint32_t *wxi = s->tmp0.as<uint32_t>(), *wxiw = s->tmp1.as<uint32_t>();
-      CS_LAUNCH(k_plonk_wxi_numerator<FrP>, ceil_div(n + 6, 128), 128, 0, st, li, W, n, pub, wxi);
-      CS_TRY(divide_by_linear<Cfg>(ctx, s, wxi, n + 6, xi, (const HR*)nullptr));
-      CS_CUDA(cudaMemcpyAsync(wxiw, s->polyadd[3].as<uint32_t>(), (size_t)(n + 3) * 32, cudaMemcpyDeviceToDevice, st));
-      CS_TRY(divide_by_linear<Cfg>(ctx, s, wxiw, n + 3, xiw, pub ? &ezw : (const HR*)nullptr));
-      Commit c[2] = {{wxi, (size_t)n + 5, h_out}, {wxiw, (size_t)n + 2, h_out + pl}};
-      return commit_many<Cfg>(ctx, pk, c, 2);
+      // the public polynomials and constants enter once (add_with_public on x_0)
+      return opening_polys<Cfg>(ctx, pk, ws, s->polyadd, s->pub.data(), s->K, in[0], in[1], in + 2, s->party == 0, h_out);
     }
     default:
       return fail(CS_ERR_ARG, "cs_plonk_rep3_step: unknown step %d", step);
@@ -853,33 +889,27 @@ int r3_prove_t(cs_plonk_rep3* s, cs_net* net, cs_rep3_state* state, const uint64
     ~Advance() { cs_rep3_state_advance(st, cs_plonk_rep3_prf_words(s)); }
   } advance{s, state};
 
-  auto open_points = [&](uint64_t* p, int k) -> int {  // open_point_vec_g1: every party adds the three partial points
-    std::vector<uint64_t> a(k * pl), b(k * pl);
-    CS_TRY(cs_net_send(net, nx, p, k * pl * 8));
-    CS_TRY(cs_net_send(net, pv, p, k * pl * 8));
-    CS_TRY(cs_net_recv(net, pv, a.data(), k * pl * 8));
-    CS_TRY(cs_net_recv(net, nx, b.data(), k * pl * 8));
-    for (int i = 0; i < k; i++) {
-      A1 x, y, z;
-      memcpy(&x, p + i * pl, sizeof(x)); memcpy(&y, a.data() + i * pl, sizeof(y)); memcpy(&z, b.data() + i * pl, sizeof(z));
-      A1 r = host::haffine(host::hadd(host::hadd(X1::from_affine(x), X1::from_affine(y)), X1::from_affine(z)));
-      memcpy(p + i * pl, &r, sizeof(r));
-    }
+  // open_point_vec_g1 / open_vec: every party sends its k partial values (`len` limbs each) to both others, then adds
+  auto open = [&](uint64_t* v, int k, size_t len, auto add) -> int {
+    std::vector<uint64_t> a(k * len), b(k * len);
+    CS_TRY(cs_net_send(net, nx, v, k * len * 8));
+    CS_TRY(cs_net_send(net, pv, v, k * len * 8));
+    CS_TRY(cs_net_recv(net, pv, a.data(), k * len * 8));
+    CS_TRY(cs_net_recv(net, nx, b.data(), k * len * 8));
+    for (int i = 0; i < k; i++) add(v + i * len, a.data() + i * len, b.data() + i * len);
     return 0;
   };
-  auto open_scalars = [&](uint64_t* v, int k) -> int {  // open_vec on a handful of values
-    std::vector<uint64_t> a(k * HR::N), b(k * HR::N);
-    CS_TRY(cs_net_send(net, nx, v, k * HR::N * 8));
-    CS_TRY(cs_net_send(net, pv, v, k * HR::N * 8));
-    CS_TRY(cs_net_recv(net, pv, a.data(), k * HR::N * 8));
-    CS_TRY(cs_net_recv(net, nx, b.data(), k * HR::N * 8));
-    for (int i = 0; i < k; i++) {
-      HR x, y, z;
-      memcpy(x.l, v + i * HR::N, sizeof(x.l)); memcpy(y.l, a.data() + i * HR::N, sizeof(y.l)); memcpy(z.l, b.data() + i * HR::N, sizeof(z.l));
-      x = x + y + z;
-      memcpy(v + i * HR::N, x.l, sizeof(x.l));
-    }
-    return 0;
+  auto add_points = [](uint64_t* x, const uint64_t* y, const uint64_t* z) {
+    A1 p[3];
+    memcpy(&p[0], x, sizeof(A1)); memcpy(&p[1], y, sizeof(A1)); memcpy(&p[2], z, sizeof(A1));
+    p[0] = host::haffine(host::hadd(host::hadd(X1::from_affine(p[0]), X1::from_affine(p[1])), X1::from_affine(p[2])));
+    memcpy(x, &p[0], sizeof(A1));
+  };
+  auto add_scalars = [](uint64_t* x, const uint64_t* y, const uint64_t* z) {
+    HR s[3];
+    memcpy(s[0].l, x, sizeof(s[0].l)); memcpy(s[1].l, y, sizeof(s[1].l)); memcpy(s[2].l, z, sizeof(s[2].l));
+    s[0] = s[0] + s[1] + s[2];
+    memcpy(x, s[0].l, sizeof(s[0].l));
   };
   void *d_out_v = nullptr, *d_in_v = nullptr;
   CS_TRY(cs_plonk_rep3_io(s, &d_out_v, &d_in_v));
@@ -937,24 +967,16 @@ int r3_prove_t(cs_plonk_rep3* s, cs_net* net, cs_rep3_state* state, const uint64
     return rc;
   };
   auto step = [&](int st, const uint64_t* in, uint64_t* out) { return cs_plonk_rep3_step(s, st, in, out); };
-  auto scalar = [](const uint64_t* p) { HR v; memcpy(v.l, p, sizeof(v.l)); return v; };
 
   uint64_t* pts = out_points;  // A B C Z T1 T2 T3 Wxi Wxiw
   // ---- round 1
   CS_TRY(cs_plonk_rep3_round1(s, &prf, h_pub, n_pub, h_wit, n_wit, blind, pts));
-  CS_TRY(open_points(pts, 3));
-  // ---- round 2 (challenges: round2.rs:226-245)
-  Transcript<Cfg> t;
-  for (int i = 0; i < 8; i++) t.add_point(pk->vk_points.data() + i * pl);
-  for (size_t i = 1; i < n_pub; i++) t.add_scalar(scalar(h_pub + i * HR::N));
-  for (int i = 0; i < 3; i++) t.add_point(pts + i * pl);
-  const HR beta = t.get_challenge();
-  t = Transcript<Cfg>();
-  t.add_scalar(beta);
-  const HR gamma = t.get_challenge();
-  uint64_t bg[2 * HR::N];
-  memcpy(bg, beta.l, sizeof(beta.l)); memcpy(bg + HR::N, gamma.l, sizeof(gamma.l));
-  CS_TRY(step(CS_PLONK_R3_ROUND2_A, bg, nullptr)); CS_TRY(reshare({0, 1}, n));
+  CS_TRY(open(pts, 3, pl, add_points));
+  // ---- round 2
+  Challenges<Cfg> ch;
+  ch.round2(pk, h_pub, pts);
+  const HR bg[2] = {ch.beta, ch.gamma};
+  CS_TRY(step(CS_PLONK_R3_ROUND2_A, bg[0].l, nullptr)); CS_TRY(reshare({0, 1}, n));
   CS_TRY(step(CS_PLONK_R3_ROUND2_B, nullptr, nullptr)); CS_TRY(reshare({2, 3}, n));
   CS_TRY(step(CS_PLONK_R3_ROUND2_C, nullptr, nullptr));
   CS_TRY(open_device_vector(2 * n + 1));
@@ -963,37 +985,25 @@ int r3_prove_t(cs_plonk_rep3* s, cs_net* net, cs_rep3_state* state, const uint64
   CS_TRY(step(CS_PLONK_R3_ROUND2_F, nullptr, nullptr));
   CS_TRY(open_device_vector(n));
   CS_TRY(step(CS_PLONK_R3_ROUND2_G, nullptr, pts + 3 * pl));
-  CS_TRY(open_points(pts + 3 * pl, 1));
+  CS_TRY(open(pts + 3 * pl, 1, pl, add_points));
   // ---- round 3
-  t = Transcript<Cfg>();
-  t.add_scalar(beta); t.add_scalar(gamma); t.add_point(pts + 3 * pl);
-  const HR alpha = t.get_challenge();
-  CS_TRY(step(CS_PLONK_R3_ROUND3_A, alpha.l, nullptr));
+  ch.round3(pts + 3 * pl);
+  CS_TRY(step(CS_PLONK_R3_ROUND3_A, ch.alpha.l, nullptr));
   CS_TRY(reshare({0, 1, 2, 3, 4, 5, 6, 7, 8, 9, 10, 11}, 4 * n));
   CS_TRY(step(CS_PLONK_R3_ROUND3_B, nullptr, pts + 4 * pl));
-  CS_TRY(open_points(pts + 4 * pl, 3));
+  CS_TRY(open(pts + 4 * pl, 3, pl, add_points));
   // ---- round 4
-  t = Transcript<Cfg>();
-  t.add_scalar(alpha);
-  for (int i = 4; i < 7; i++) t.add_point(pts + i * pl);
-  const HR xi = t.get_challenge();
-  uint64_t ev[6 * HR::N];  // partial a b c zw | public s1 s2
-  CS_TRY(step(CS_PLONK_R3_ROUND4, xi.l, ev));
-  CS_TRY(open_scalars(ev, 4));
-  const HR ea = scalar(ev), eb = scalar(ev + HR::N), ec = scalar(ev + 2 * HR::N), ezw = scalar(ev + 3 * HR::N),
-           es1 = scalar(ev + 4 * HR::N), es2 = scalar(ev + 5 * HR::N);
+  ch.round4(pts + 4 * pl);
+  HR e[6];  // partial a b c zw | public s1 s2
+  CS_TRY(step(CS_PLONK_R3_ROUND4, ch.xi.l, e[0].l));
+  CS_TRY(open(e[0].l, 4, HR::N, add_scalars));
   // ---- round 5
-  t = Transcript<Cfg>();
-  const HR order[7] = {xi, ea, eb, ec, es1, es2, ezw};
-  for (const HR& x : order) t.add_scalar(x);
-  const HR v0 = t.get_challenge();
-  const HR in5[8] = {xi, v0, ea, eb, ec, es1, es2, ezw};
-  uint64_t in5l[8 * HR::N];
-  for (int i = 0; i < 8; i++) memcpy(in5l + i * HR::N, in5[i].l, sizeof(in5[i].l));
-  CS_TRY(step(CS_PLONK_R3_ROUND5, in5l, pts + 7 * pl));
-  CS_TRY(open_points(pts + 7 * pl, 2));
-  const HR evs[6] = {ea, eb, ec, es1, es2, ezw};
-  for (int i = 0; i < 6; i++) memcpy(out_evals + i * HR::N, evs[i].l, sizeof(evs[i].l));
+  const HR ev[6] = {e[0], e[1], e[2], e[4], e[5], e[3]};  // the proof's order: a b c s1 s2 zw
+  ch.round5(ev);
+  const HR in5[8] = {ch.xi, ch.v, ev[0], ev[1], ev[2], ev[3], ev[4], ev[5]};
+  CS_TRY(step(CS_PLONK_R3_ROUND5, in5[0].l, pts + 7 * pl));
+  CS_TRY(open(pts + 7 * pl, 2, pl, add_points));
+  memcpy(out_evals, ev, sizeof(ev));
   return 0;
 }
 
@@ -1018,35 +1028,20 @@ struct cs_plonk_shamir {
   cs_plonk_pk* pk = nullptr;
   int n_parties = 0, thr = 0, party = 0;
   cs_shamir_state* state = nullptr;  // created over the first proof's net, kept for the next ones
-  DevBuf w, buf[3], poly[4], ev[4], arena, pair_t, pair_2t, addv, pubv, t, tz, t1, t2, t3, tmp0, tmp1, totals, small;
+  PlonkWork ws;
+  DevBuf arena, pair_t, pair_2t, addv, pubv;
   size_t pairs = 0;    // pairs the last proof consumed
   double pair_ms = 0;  // wall time of the last proof's device pair generation
 };
 
 namespace {
 
-template <class Cfg>
-int sh_create_t(cs_plonk_shamir* s) {
-  const cs_plonk_pk* pk = s->pk;
-  const size_t n = pk->n;
-  CS_TRY(s->w.reserve((size_t)pk->n_vars * 32));
-  for (int i = 0; i < 3; i++) CS_TRY(s->buf[i].reserve(n * 32));
-  for (int i = 0; i < 4; i++) {
-    CS_TRY(s->poly[i].reserve((n + 8) * 32));
-    CS_TRY(s->ev[i].reserve(4 * n * 32));
-  }
+int sh_create(cs_plonk_shamir* s) {
+  const size_t n = s->pk->n;
+  CS_TRY(s->ws.reserve(n, s->pk->n_vars, 1));
   CS_TRY(s->arena.reserve(48 * n * 32));  // round 3: twelve slots of 4n; round 2: seven slots of n
   CS_TRY(s->addv.reserve((2 * n + 2) * 32));
-  CS_TRY(s->pubv.reserve((8 * n + 16) * 32));  // 1/G | 1/Q | scan scratch | opened G | Q
-  CS_TRY(s->t.reserve(4 * n * 32));
-  CS_TRY(s->tz.reserve(4 * n * 32));
-  CS_TRY(s->t1.reserve((n + 8) * 32));
-  CS_TRY(s->t2.reserve((n + 8) * 32));
-  CS_TRY(s->t3.reserve((n + 8) * 32));
-  CS_TRY(s->tmp0.reserve((n + 8) * 32));
-  CS_TRY(s->tmp1.reserve((n + 8) * 32));
-  CS_TRY(s->small.reserve(8192));
-  return 0;
+  return s->pubv.reserve((8 * n + 16) * 32);  // 1/G | 1/Q | scan scratch | opened G | Q
 }
 
 template <class Cfg>
@@ -1058,9 +1053,10 @@ int sh_prove_t(cs_plonk_shamir* s, cs_net* net, const uint64_t* h_pub, const uin
   constexpr int NW = FrP::N;
   cs_ctx* ctx = s->ctx;
   cs_plonk_pk* pk = s->pk;
+  PlonkWork& ws = s->ws;
   cudaStream_t st = ctx->stream;
   const cs_curve cv = (cs_curve)pk->curve;
-  const uint32_t n = pk->n, n4 = 4 * n, npub = pk->n_public;
+  const uint32_t n = pk->n, n4 = 4 * n;
   const size_t pl = point_limbs64(pk->curve, CS_G1);
   const unsigned gb = ceil_div(n, 128);
   s->pairs = 0;
@@ -1092,58 +1088,19 @@ int sh_prove_t(cs_plonk_shamir* s, cs_net* net, const uint64_t* h_pub, const uin
   auto open_points = [&](uint64_t* p, int k, int degree_2t) {
     return shamir_open_points(sst, net, CS_G1, degree_2t, p, k);
   };
-  // ---- init round (round1.rs:191-252): w = 0 | public (every party holds the value itself) | witness shares | additions
-  uint32_t* w = s->w.as<uint32_t>();
-  const uint32_t n_priv = pk->n_vars - pk->n_additions - npub - 1;
-  CS_CUDA(cudaMemsetAsync(w, 0, 32, st));
-  if (npub) CS_CUDA(cudaMemcpyAsync(w + NW, h_pub + HR::N, (size_t)npub * 32, cudaMemcpyHostToDevice, st));
-  if (n_priv) CS_CUDA(cudaMemcpyAsync(w + (size_t)(npub + 1) * NW, h_wit, (size_t)n_priv * 32, cudaMemcpyHostToDevice, st));
-  {
-    uint32_t lo = 0;
-    for (uint32_t hi : pk->level_ends) {
-      CS_LAUNCH(k_plonk_additions<FrP>, ceil_div(hi - lo, 128), 128, 0, st, pk->add_order.as<uint32_t>(), lo, hi,
-                pk->add_ids.as<uint32_t>(), pk->add_factors.as<uint32_t>(), pk->n_vars - pk->n_additions, 1u, w);
-      lo = hi;
-    }
-  }
-  // ---- round 1
-  const uint32_t* maps[3] = {pk->map_a.as<uint32_t>(), pk->map_b.as<uint32_t>(), pk->map_c.as<uint32_t>()};
-  uint32_t *buf[3], *poly[4], *ev[4];
-  for (int i = 0; i < 3; i++) buf[i] = s->buf[i].as<uint32_t>();
-  for (int i = 0; i < 4; i++) { poly[i] = s->poly[i].as<uint32_t>(); ev[i] = s->ev[i].as<uint32_t>(); }
-  for (int k = 0; k < 3; k++) {
-    CS_LAUNCH(k_plonk_gather<FrP>, ceil_div(n, 256), 256, 0, st, maps[k], pk->n_constraints, n, 1u, w, buf[k]);
-    CS_CUDA(cudaMemcpyAsync(poly[k], buf[k], (size_t)n * 32, cudaMemcpyDeviceToDevice, st));
-    CS_TRY(interpolate_and_extend<Cfg>(ctx, pk, poly[k], ev[k]));
-    CS_TRY(blind<Cfg>(ctx, poly[k], n, b + 2 * k, 2));
-  }
   uint64_t* P = out_points;  // A B C Z T1 T2 T3 Wxi Wxiw
-  {
-    Commit c[3] = {{poly[0], (size_t)n + 2, P}, {poly[1], (size_t)n + 2, P + pl}, {poly[2], (size_t)n + 2, P + 2 * pl}};
-    CS_TRY(commit_many<Cfg>(ctx, pk, c, 3));
-  }
+  // ---- init round (every party holds the public values themselves), round 1
+  CS_TRY(load_witness<Cfg>(ctx, pk, ws, h_pub, h_wit, 1, 0));
+  for (int k = 0; k < 3; k++) CS_TRY(wire_poly<Cfg>(ctx, pk, ws, k, 1, b + 2 * k));
+  CS_TRY(commit_polys<Cfg>(ctx, pk, ws.poly, 3, (size_t)n + 2, P));
   CS_TRY(open_points(P, 3, 0));
   // ---- round 2 (round2.rs:197-250)
-  HR k1, k2;
-  memcpy(k1.l, pk->k1.data(), sizeof(k1.l));
-  memcpy(k2.l, pk->k2.data(), sizeof(k2.l));
-  Transcript<Cfg> tr;
-  for (int i = 0; i < 8; i++) tr.add_point(pk->vk_points.data() + i * pl);
-  for (uint32_t i = 0; i < npub; i++) {
-    HR v;
-    memcpy(v.l, h_pub + (size_t)(i + 1) * HR::N, sizeof(v.l));
-    tr.add_scalar(v);
-  }
-  for (int i = 0; i < 3; i++) tr.add_point(P + i * pl);
-  const HR beta = tr.get_challenge();
-  tr = Transcript<Cfg>();
-  tr.add_scalar(beta);
-  const HR gamma = tr.get_challenge();
+  Challenges<Cfg> ch;
+  ch.round2(pk, h_pub, P);
   PlonkConsts K;
-  memset(&K, 0, sizeof(K));
-  for (int i = 0; i < 11; i++) put(K.b[i], b[i]);
-  put(K.beta, beta); put(K.gamma, gamma); put(K.k1, k1); put(K.k2, k2);
-  const uint32_t* tw4 = pk->dom4->tw_fwd.template as<uint32_t>();
+  init_consts<Cfg>(K, pk, b, 1);
+  put(K.beta, ch.beta);
+  put(K.gamma, ch.gamma);
   CS_TRY(make_pairs(10 * (size_t)n + 2));
   const ShamirRnd R{s->pair_t.as<uint32_t>()};  // s, r, s' = the r_t halves of pairs [0, 3n + 2)
   const size_t first = 3 * (size_t)n + 2;         // the reductions take the pairs after them
@@ -1152,10 +1109,7 @@ int sh_prove_t(cs_plonk_shamir* s, cs_net* net, const uint64_t* h_pub, const uin
   uint32_t *pubv = s->pubv.as<uint32_t>(), *addv = s->addv.as<uint32_t>();
   uint32_t *ginv = pubv, *qinv = pubv + (size_t)n * NW, *pscr = pubv + (size_t)(2 * n + 1) * NW;
   uint32_t* opened = pscr + (size_t)(4 * n + 4) * NW;
-  R3Round2In in;
-  in.a = buf[0]; in.b = buf[1]; in.c = buf[2];
-  in.s1 = pk->s_evals[0].as<uint32_t>(); in.s2 = pk->s_evals[1].as<uint32_t>(); in.s3 = pk->s_evals[2].as<uint32_t>();
-  in.tw4 = tw4;
+  const R3Round2In in = r3_round2_in(pk, ws);
   uint32_t* none = nullptr;
   CS_LAUNCH(k_r3_round2_a<Pol>, gb, 128, 0, st, in, K, n, s->party, R, 0ull, slot(0), slot(1), none, none);
   CS_TRY(reduce(slot(0), 2 * (size_t)n, first));
@@ -1164,8 +1118,8 @@ int sh_prove_t(cs_plonk_shamir* s, cs_net* net, const uint64_t* h_pub, const uin
   CS_LAUNCH(k_r3_round2_c<Pol>, ceil_div(n + 1, 128), 128, 0, st, slot(3), n, R, 0ull, 0ull, addv, addv + (size_t)n * NW);
   CS_CUDA(cudaStreamSynchronize(st));
   CS_TRY(shamir_open_vec(ctx, sst, net, 1, (const uint64_t*)addv, 2 * (size_t)n + 1, (uint64_t*)opened));
-  CS_TRY(r3_batch_inverse<Cfg>(s, opened, n, pscr, ginv));
-  CS_TRY(r3_batch_inverse<Cfg>(s, opened + (size_t)n * NW, n + 1, pscr, qinv));
+  CS_TRY(r3_batch_inverse<Cfg>(ctx, ws, opened, n, pscr, ginv));
+  CS_TRY(r3_batch_inverse<Cfg>(ctx, ws, opened + (size_t)n * NW, n + 1, pscr, qinv));
   CS_LAUNCH(k_r3_round2_d<Pol>, gb, 128, 0, st, slot(2), ginv, qinv, n, R, 0ull, 0ull, slot(4), slot(5), none, none);
   CS_TRY(reduce(slot(4), 2 * (size_t)n, first + 4 * (size_t)n));
   CS_LAUNCH(k_r3_round2_e<Pol>, gb, 128, 0, st, slot(4), n, R, 0ull, 0ull, slot(6), none);
@@ -1174,27 +1128,16 @@ int sh_prove_t(cs_plonk_shamir* s, cs_net* net, const uint64_t* h_pub, const uin
   CS_CUDA(cudaStreamSynchronize(st));
   uint32_t* y = pscr;
   CS_TRY(shamir_open_vec(ctx, sst, net, 1, (const uint64_t*)addv, n, (uint64_t*)y));
-  CS_TRY((scan<FrP, 0>(ctx, s, y, y, n, 0)));
-  CS_LAUNCH(k_r3_round2_g<Pol>, gb, 128, 0, st, y, slot(5), n, poly[3]);
-  CS_TRY(interpolate_and_extend<Cfg>(ctx, pk, poly[3], ev[3]));
-  CS_TRY(blind<Cfg>(ctx, poly[3], n, b + 6, 3));
-  {
-    Commit c[1] = {{poly[3], (size_t)n + 3, P + 3 * pl}};
-    CS_TRY(commit_many<Cfg>(ctx, pk, c, 1));
-  }
+  CS_TRY((scan<FrP, 0>(ctx, ws, y, y, n, 0)));
+  CS_LAUNCH(k_r3_round2_g<Pol>, gb, 128, 0, st, y, slot(5), n, ws.poly[3].as<uint32_t>());
+  CS_TRY(z_poly<Cfg>(ctx, pk, ws, 1, b + 6));
+  CS_TRY(commit_polys<Cfg>(ctx, pk, ws.poly + 3, 1, (size_t)n + 3, P + 3 * pl));
   CS_TRY(open_points(P + 3 * pl, 1, 0));
   // ---- round 3 (round3.rs:560-610)
-  tr = Transcript<Cfg>();
-  tr.add_scalar(beta);
-  tr.add_scalar(gamma);
-  tr.add_point(P + 3 * pl);
-  const HR alpha = tr.get_challenge();
-  const HR alpha2 = alpha.sqr();
-  put(K.alpha, alpha); put(K.alpha2, alpha2);
-  CS_TRY(quotient_consts<Cfg>(pk->curve, K));
+  ch.round3(P + 3 * pl);
+  CS_TRY(set_alpha<Cfg>(pk, K, ch.alpha));
   CS_TRY(make_pairs(48 * (size_t)n));
-  R3QuotIn qi;
-  qi.a = ev[0]; qi.b = ev[1]; qi.c = ev[2]; qi.z = ev[3]; qi.tw4 = tw4;
+  const R3QuotIn qi = r3_quot_in(pk, ws);
   R3Blinders B;
   memset(&B, 0, sizeof(B));
   for (int i = 0; i < 9; i++) put(B.b[i].v[0], b[i]);
@@ -1202,64 +1145,31 @@ int sh_prove_t(cs_plonk_shamir* s, cs_net* net, const uint64_t* h_pub, const uin
   const ShamirRnd R3{nullptr};  // round 3 draws no random shares; round 2's pair buffer has been replaced
   CS_LAUNCH(k_r3_quot_l1<Pol>, ceil_div(n4, 64), 64, 0, st, qi, B, n, R3, 0ull, arena, none, slot_words);
   CS_TRY(reduce(arena, 12 * (size_t)n4, 0));
-  R3KeyEvals E;
-  E.qm = pk->q_evals[0].as<uint32_t>(); E.ql = pk->q_evals[1].as<uint32_t>(); E.qr = pk->q_evals[2].as<uint32_t>();
-  E.qo = pk->q_evals[3].as<uint32_t>(); E.qc = pk->q_evals[4].as<uint32_t>();
-  E.s1 = pk->s_evals[0].as<uint32_t>(); E.s2 = pk->s_evals[1].as<uint32_t>(); E.s3 = pk->s_evals[2].as<uint32_t>();
-  E.lagrange = pk->lagrange.as<uint32_t>(); E.buf_a = buf[0];
-  uint32_t *t = s->t.as<uint32_t>(), *tz = s->tz.as<uint32_t>();
-  CS_LAUNCH(k_r3_quot_l2<Pol>, ceil_div(n4, 64), 64, 0, st, qi, B, E, n, pk->nlag, K, s->party, R3, 0ull, arena, slot_words, t, tz);
-  CS_TRY(ntt_run(ctx, pk->dom4, t, 1, true, nullptr, st));
-  CS_TRY(ntt_run(ctx, pk->dom4, tz, 1, true, nullptr, st));
-  CS_LAUNCH(k_bit_reverse<FrP>, ceil_div(n4, 256), 256, 0, st, t, pk->log_n + 2, 1u);
-  CS_LAUNCH(k_bit_reverse<FrP>, ceil_div(n4, 256), 256, 0, st, tz, pk->log_n + 2, 1u);
-  uint32_t *t1 = s->t1.as<uint32_t>(), *t2 = s->t2.as<uint32_t>(), *t3 = s->t3.as<uint32_t>();
-  CS_LAUNCH(k_plonk_tsplit<FrP>, gb, 128, 0, st, t, tz, n, K, t1, t2, t3);
-  {
-    Commit c[3] = {{t1, (size_t)n + 1, P + 4 * pl}, {t2, (size_t)n + 1, P + 5 * pl}, {t3, (size_t)n + 6, P + 6 * pl}};
-    CS_TRY(commit_many<Cfg>(ctx, pk, c, 3));
-  }
+  CS_LAUNCH(k_r3_quot_l2<Pol>, ceil_div(n4, 64), 64, 0, st, qi, B, key_evals(pk, ws), n, pk->nlag, K, s->party, R3, 0ull, arena,
+            slot_words, ws.t.as<uint32_t>(), ws.tz.as<uint32_t>());
+  CS_TRY(split_and_commit<Cfg>(ctx, pk, ws, K, P + 4 * pl));
   CS_TRY(open_points(P + 4 * pl, 3, 1));
-  // ---- round 4 (round4.rs:108-165)
-  tr = Transcript<Cfg>();
-  tr.add_scalar(alpha);
-  for (int i = 4; i < 7; i++) tr.add_point(P + i * pl);
-  const HR xi = tr.get_challenge();
-  HR w_n;
-  memcpy(w_n.l, pk->dom->group_gen.data(), sizeof(w_n.l));
-  const HR xiw = xi * w_n;
-  HR ev4[4], es1, es2;  // a b c zw (shares, then opened)
-  for (int k = 0; k < 3; k++) CS_TRY((eval_poly_t<Cfg>(ctx, reinterpret_cast<uint64_t*>(poly[k]), (size_t)n + 2, 1, xi.l, ev4[k].l)));
-  CS_TRY((eval_poly_t<Cfg>(ctx, reinterpret_cast<uint64_t*>(poly[3]), (size_t)n + 3, 1, xiw.l, ev4[3].l)));
-  CS_TRY((eval_poly_t<Cfg>(ctx, pk->s_coeffs[0].as<uint64_t>(), (size_t)n, 1, xi.l, es1.l)));
-  CS_TRY((eval_poly_t<Cfg>(ctx, pk->s_coeffs[1].as<uint64_t>(), (size_t)n, 1, xi.l, es2.l)));
-  CS_TRY(shamir_open_scalars(sst, net, 0, ev4[0].l, 4));
-  const HR ea = ev4[0], eb = ev4[1], ec = ev4[2], ezw = ev4[3];
-  // ---- round 5 (round5.rs:284-340)
-  tr = Transcript<Cfg>();
-  tr.add_scalar(xi); tr.add_scalar(ea); tr.add_scalar(eb); tr.add_scalar(ec);
-  tr.add_scalar(es1); tr.add_scalar(es2); tr.add_scalar(ezw);
-  const HR evs5[6] = {ea, eb, ec, es1, es2, ezw};
-  PlonkLinW W;
-  CS_TRY(lin_weights<Cfg>(pk, h_pub + HR::N, K, xi, tr.get_challenge(), evs5, W));
-  PlonkLinIn li;
-  li.qm = pk->q_coeffs[0].as<uint32_t>(); li.ql = pk->q_coeffs[1].as<uint32_t>(); li.qr = pk->q_coeffs[2].as<uint32_t>();
-  li.qo = pk->q_coeffs[3].as<uint32_t>(); li.qc = pk->q_coeffs[4].as<uint32_t>();
-  li.s1 = pk->s_coeffs[0].as<uint32_t>(); li.s2 = pk->s_coeffs[1].as<uint32_t>(); li.s3 = pk->s_coeffs[2].as<uint32_t>();
-  li.pa = poly[0]; li.pb = poly[1]; li.pc = poly[2]; li.pz = poly[3]; li.t1 = t1; li.t2 = t2; li.t3 = t3;
-  uint32_t *wxi = s->tmp0.as<uint32_t>(), *wxiw = s->tmp1.as<uint32_t>();
-  CS_LAUNCH(k_plonk_wxi_numerator<FrP>, ceil_div(n + 6, 128), 128, 0, st, li, W, n, 1, wxi);  // pub = 1 at every party
-  CS_TRY(divide_by_linear<Cfg>(ctx, s, wxi, n + 6, xi, (const HR*)nullptr));
-  CS_CUDA(cudaMemcpyAsync(wxiw, poly[3], (size_t)(n + 3) * 32, cudaMemcpyDeviceToDevice, st));
-  CS_TRY(divide_by_linear<Cfg>(ctx, s, wxiw, n + 3, xiw, &ezw));
-  {
-    Commit c[2] = {{wxi, (size_t)n + 5, P + 7 * pl}, {wxiw, (size_t)n + 2, P + 8 * pl}};
-    CS_TRY(commit_many<Cfg>(ctx, pk, c, 2));
-  }
+  // ---- round 4
+  ch.round4(P + 4 * pl);
+  HR e[6];  // a b c zw (shares, then opened) | public s1 s2
+  CS_TRY(evaluate<Cfg>(ctx, pk, ws.poly, ch.xi, e[0].l));
+  CS_TRY(shamir_open_scalars(sst, net, 0, e[0].l, 4));
+  // ---- round 5
+  const HR ev[6] = {e[0], e[1], e[2], e[4], e[5], e[3]};  // the proof's order: a b c s1 s2 zw
+  ch.round5(ev);
+  CS_TRY(opening_polys<Cfg>(ctx, pk, ws, ws.poly, h_pub + HR::N, K, ch.xi, ch.v, ev, 1, P + 7 * pl));  // public terms at every party
   CS_TRY(open_points(P + 7 * pl, 1, 1));  // Wxi: degree 2t (it carries T1 T2 T3)
   CS_TRY(open_points(P + 8 * pl, 1, 0));  // Wxiw: degree t
-  const HR evs[6] = {ea, eb, ec, es1, es2, ezw};
-  memcpy(out_evals, evs, sizeof(evs));
+  memcpy(out_evals, ev, sizeof(ev));
+  return 0;
+}
+
+// the caller's public inputs (the leading one included) and witness entries against the key
+int check_counts(const cs_plonk_pk* pk, size_t n_public_inputs, size_t n_witness, const char* fn) {
+  if (n_public_inputs != (size_t)pk->n_public + 1)
+    return fail(CS_ERR_ARG, "%s: %zu public inputs, the key expects %u (incl. the leading one)", fn, n_public_inputs,
+                pk->n_public + 1);
+  if (n_witness != pk->n_witness()) return fail(CS_ERR_ARG, "%s: %zu witness values, the key expects %u", fn, n_witness, pk->n_witness());
   return 0;
 }
 
@@ -1280,14 +1190,8 @@ int cs_plonk_pk_create(cs_ctx* ctx, const cs_plonk_key_desc* d, cs_plonk_pk** ou
   CS_CUDA(cudaSetDevice(ctx->device));
   std::unique_ptr<cs_plonk_pk> pk(new cs_plonk_pk());
   pk->curve = d->curve;
-  int rc;
-  switch ((int)d->curve) {
-    case CS_BN254: rc = plonk_pk_create_t<Bn254Cfg>(ctx, d, pk.get()); break;
-#if defined(CS_ENABLE_BLS12_381)
-    case CS_BLS12_381: rc = plonk_pk_create_t<Bls381Cfg>(ctx, d, pk.get()); break;
-#endif
-    default: rc = fail(CS_ERR_ARG, "unsupported curve id %d", (int)d->curve);
-  }
+  int rc = 0;
+  CS_DISPATCH_CURVE(d->curve, rc = plonk_pk_create_t<Cfg>(ctx, d, pk.get()));
   if (rc) {
     cs_plonk_pk_free(pk.release());
     return rc;
@@ -1301,12 +1205,11 @@ void cs_plonk_pk_free(cs_plonk_pk* pk) {
   cs_bases_free(pk->p_tau);
   cs_domain_free(pk->dom);
   cs_domain_free(pk->dom4);
-  DevBuf* all[] = {&pk->add_ids, &pk->add_factors, &pk->add_order, &pk->map_a, &pk->map_b, &pk->map_c, &pk->lagrange, &pk->w,
-                   &pk->t, &pk->tz, &pk->t1, &pk->t2, &pk->t3, &pk->tmp0, &pk->tmp1, &pk->totals, &pk->small};
+  DevBuf* all[] = {&pk->add_ids, &pk->add_factors, &pk->add_order, &pk->map_a, &pk->map_b, &pk->map_c, &pk->lagrange};
   for (DevBuf* b : all) b->release();
   for (int i = 0; i < 5; i++) { pk->q_coeffs[i].release(); pk->q_evals[i].release(); }
-  for (int i = 0; i < 3; i++) { pk->s_coeffs[i].release(); pk->s_evals[i].release(); pk->buf[i].release(); }
-  for (int i = 0; i < 4; i++) { pk->poly[i].release(); pk->ev[i].release(); }
+  for (int i = 0; i < 3; i++) { pk->s_coeffs[i].release(); pk->s_evals[i].release(); }
+  pk->ws.release();
   delete pk;
 }
 
@@ -1315,7 +1218,7 @@ int cs_plonk_pk_curve(const cs_plonk_pk* pk) { return pk ? pk->curve : CS_ERR_AR
 int cs_plonk_pk_info(const cs_plonk_pk* pk, size_t* n_public, size_t* n_witness, size_t* domain_size, uint64_t* vk_points) {
   if (!pk) return fail(CS_ERR_ARG, "cs_plonk_pk_info: NULL key");
   if (n_public) *n_public = pk->n_public;
-  if (n_witness) *n_witness = (size_t)pk->n_vars - pk->n_additions - pk->n_public - 1;
+  if (n_witness) *n_witness = pk->n_witness();
   if (domain_size) *domain_size = pk->n;
   if (vk_points) memcpy(vk_points, pk->vk_points.data(), pk->vk_points.size() * 8);
   return 0;
@@ -1333,19 +1236,9 @@ int cs_plonk_prove_plain(cs_ctx* ctx, cs_plonk_pk* pk, const uint64_t* h_public_
                          uint64_t* out_points, uint64_t* out_evals) {
   if (!ctx || !pk || !h_public_inputs || !h_blinders_mont || !out_points || !out_evals || (n_witness && !h_witness))
     return fail(CS_ERR_ARG, "cs_plonk_prove_plain: NULL argument");
-  if (n_public_inputs != (size_t)pk->n_public + 1)
-    return fail(CS_ERR_ARG, "cs_plonk_prove_plain: %zu public inputs, the key expects %u (incl. the leading one)",
-                n_public_inputs, pk->n_public + 1);
-  if (n_witness != (size_t)pk->n_vars - pk->n_additions - pk->n_public - 1)
-    return fail(CS_ERR_ARG, "cs_plonk_prove_plain: %zu witness values, the key expects %u", n_witness,
-                pk->n_vars - pk->n_additions - pk->n_public - 1);
-  switch (pk->curve) {
-    case CS_BN254: return plonk_prove_plain_t<Bn254Cfg>(ctx, pk, h_public_inputs, h_witness, h_blinders_mont, out_points, out_evals);
-#if defined(CS_ENABLE_BLS12_381)
-    case CS_BLS12_381: return plonk_prove_plain_t<Bls381Cfg>(ctx, pk, h_public_inputs, h_witness, h_blinders_mont, out_points, out_evals);
-#endif
-    default: return fail(CS_ERR_ARG, "unsupported curve id %d", pk->curve);
-  }
+  CS_TRY(check_counts(pk, n_public_inputs, n_witness, "cs_plonk_prove_plain"));
+  CS_DISPATCH_CURVE(pk->curve, return plonk_prove_plain_t<Cfg>(ctx, pk, h_public_inputs, h_witness, h_blinders_mont, out_points, out_evals));
+  return 0;
 }
 
 
@@ -1356,11 +1249,7 @@ int cs_plonk_rep3_create(cs_ctx* ctx, cs_plonk_pk* pk, int party, cs_plonk_rep3*
   std::unique_ptr<cs_plonk_rep3> s(new cs_plonk_rep3());
   s->ctx = ctx; s->pk = pk; s->party = party;
   memset(&s->prf, 0, sizeof(s->prf));
-  int rc = pk->curve == CS_BN254 ? r3_create_t<Bn254Cfg>(s.get())
-#if defined(CS_ENABLE_BLS12_381)
-           : pk->curve == CS_BLS12_381 ? r3_create_t<Bls381Cfg>(s.get())
-#endif
-           : fail(CS_ERR_ARG, "unsupported curve id %d", pk->curve);
+  const int rc = r3_create(s.get());
   if (rc) { cs_plonk_rep3_free(s.release()); return rc; }
   *out = s.release();
   return 0;
@@ -1368,10 +1257,9 @@ int cs_plonk_rep3_create(cs_ctx* ctx, cs_plonk_pk* pk, int party, cs_plonk_rep3*
 
 void cs_plonk_rep3_free(cs_plonk_rep3* s) {
   if (!s) return;
-  DevBuf* all[] = {&s->w, &s->arena, &s->addv, &s->pubv, &s->t, &s->tz, &s->t1, &s->t2, &s->t3, &s->tmp0, &s->tmp1, &s->totals, &s->small};
+  DevBuf* all[] = {&s->arena, &s->addv, &s->pubv, &s->polyadd[0], &s->polyadd[1], &s->polyadd[2], &s->polyadd[3]};
   for (DevBuf* b : all) b->release();
-  for (int i = 0; i < 3; i++) s->buf[i].release();
-  for (int i = 0; i < 4; i++) { s->polysh[i].release(); s->ev[i].release(); s->polyadd[i].release(); }
+  s->ws.release();
   delete s;
 }
 
@@ -1401,25 +1289,15 @@ int cs_plonk_rep3_round1(cs_plonk_rep3* s, const cs_rep3_prf* prf, const uint64_
                          uint64_t* out_points) {
   if (!s || !prf || !h_public_inputs || !h_blinder_shares || !out_points || (n_witness && !h_witness_shares))
     return fail(CS_ERR_ARG, "cs_plonk_rep3_round1: NULL argument");
-  const cs_plonk_pk* pk = s->pk;
-  if (n_public_inputs != (size_t)pk->n_public + 1)
-    return fail(CS_ERR_ARG, "cs_plonk_rep3_round1: %zu public inputs, the key expects %u", n_public_inputs, pk->n_public + 1);
-  if (n_witness != (size_t)pk->n_vars - pk->n_additions - pk->n_public - 1)
-    return fail(CS_ERR_ARG, "cs_plonk_rep3_round1: %zu witness shares, the key expects %u", n_witness,
-                pk->n_vars - pk->n_additions - pk->n_public - 1);
+  CS_TRY(check_counts(s->pk, n_public_inputs, n_witness, "cs_plonk_rep3_round1"));
   if (prf->rounds == 0 || (prf->rounds & 1) || prf->rounds > 20) return fail(CS_ERR_ARG, "cs_plonk_rep3_round1: bad ChaCha round count");
   CS_CUDA(cudaSetDevice(s->ctx->device));
   memcpy(s->prf.keys.k, prf->seed1, 32);
   memcpy(s->prf.keys.k + 8, prf->seed2, 32);
   s->prf.pos1 = prf->word_pos1; s->prf.pos2 = prf->word_pos2; s->prf.rounds = prf->rounds;
   s->ctr = 0;
-  switch (pk->curve) {
-    case CS_BN254: return r3_round1_t<Bn254Cfg>(s, h_public_inputs, h_witness_shares, h_blinder_shares, out_points);
-#if defined(CS_ENABLE_BLS12_381)
-    case CS_BLS12_381: return r3_round1_t<Bls381Cfg>(s, h_public_inputs, h_witness_shares, h_blinder_shares, out_points);
-#endif
-    default: return fail(CS_ERR_ARG, "unsupported curve id %d", pk->curve);
-  }
+  CS_DISPATCH_CURVE(s->pk->curve, return r3_round1_t<Cfg>(s, h_public_inputs, h_witness_shares, h_blinder_shares, out_points));
+  return 0;
 }
 
 int cs_plonk_rep3_step(cs_plonk_rep3* s, int step, const uint64_t* h_in, uint64_t* h_out) {
@@ -1434,13 +1312,8 @@ int cs_plonk_rep3_step(cs_plonk_rep3* s, int step, const uint64_t* h_in, uint64_
     if (needs_in && !h_in) return fail(CS_ERR_ARG, "cs_plonk_rep3_step: step %d reads h_in, which is NULL", step);
     if (needs_out && !h_out) return fail(CS_ERR_ARG, "cs_plonk_rep3_step: step %d writes h_out, which is NULL", step);
   }
-  switch (s->pk->curve) {
-    case CS_BN254: return r3_step_t<Bn254Cfg>(s, step, h_in, h_out);
-#if defined(CS_ENABLE_BLS12_381)
-    case CS_BLS12_381: return r3_step_t<Bls381Cfg>(s, step, h_in, h_out);
-#endif
-    default: return fail(CS_ERR_ARG, "unsupported curve id %d", s->pk->curve);
-  }
+  CS_DISPATCH_CURVE(s->pk->curve, return r3_step_t<Cfg>(s, step, h_in, h_out));
+  return 0;
 }
 
 uint64_t cs_plonk_rep3_prf_words(const cs_plonk_rep3* s) { return s ? 8 * s->ctr : 0; }
@@ -1460,13 +1333,9 @@ int cs_plonk_rep3_prove(cs_plonk_rep3* s, cs_net* net, cs_rep3_state* state, con
     return fail(CS_ERR_ARG, "cs_plonk_rep3_prove: NULL argument");
   if (net->n != 3 || net->id != s->party) return fail(CS_ERR_ARG, "cs_plonk_rep3_prove: the net is party %d of %d, the session is party %d of 3", net->id, net->n, s->party);
   CS_CUDA(cudaSetDevice(s->ctx->device));
-  switch (s->pk->curve) {
-    case CS_BN254: return r3_prove_t<Bn254Cfg>(s, net, state, h_public_inputs, n_public_inputs, h_witness_shares, n_witness, h_blinder_shares, out_points, out_evals);
-#if defined(CS_ENABLE_BLS12_381)
-    case CS_BLS12_381: return r3_prove_t<Bls381Cfg>(s, net, state, h_public_inputs, n_public_inputs, h_witness_shares, n_witness, h_blinder_shares, out_points, out_evals);
-#endif
-    default: return fail(CS_ERR_ARG, "unsupported curve id %d", s->pk->curve);
-  }
+  CS_DISPATCH_CURVE(s->pk->curve, return r3_prove_t<Cfg>(s, net, state, h_public_inputs, n_public_inputs, h_witness_shares, n_witness,
+                                                         h_blinder_shares, out_points, out_evals));
+  return 0;
 }
 
 int cs_plonk_shamir_create(cs_ctx* ctx, cs_plonk_pk* pk, int num_parties, int threshold, int party, cs_plonk_shamir** out) {
@@ -1477,11 +1346,7 @@ int cs_plonk_shamir_create(cs_ctx* ctx, cs_plonk_pk* pk, int num_parties, int th
   CS_CUDA(cudaSetDevice(ctx->device));
   std::unique_ptr<cs_plonk_shamir> s(new cs_plonk_shamir());
   s->ctx = ctx; s->pk = pk; s->n_parties = num_parties; s->thr = threshold; s->party = party;
-  int rc = pk->curve == CS_BN254 ? sh_create_t<Bn254Cfg>(s.get())
-#if defined(CS_ENABLE_BLS12_381)
-           : pk->curve == CS_BLS12_381 ? sh_create_t<Bls381Cfg>(s.get())
-#endif
-           : fail(CS_ERR_ARG, "unsupported curve id %d", pk->curve);
+  const int rc = sh_create(s.get());
   if (rc) { cs_plonk_shamir_free(s.release()); return rc; }
   *out = s.release();
   return 0;
@@ -1489,11 +1354,9 @@ int cs_plonk_shamir_create(cs_ctx* ctx, cs_plonk_pk* pk, int num_parties, int th
 
 void cs_plonk_shamir_free(cs_plonk_shamir* s) {
   if (!s) return;
-  DevBuf* all[] = {&s->w, &s->arena, &s->pair_t, &s->pair_2t, &s->addv, &s->pubv, &s->t, &s->tz, &s->t1, &s->t2, &s->t3,
-                   &s->tmp0, &s->tmp1, &s->totals, &s->small};
+  DevBuf* all[] = {&s->arena, &s->pair_t, &s->pair_2t, &s->addv, &s->pubv};
   for (DevBuf* b : all) b->release();
-  for (int i = 0; i < 3; i++) s->buf[i].release();
-  for (int i = 0; i < 4; i++) { s->poly[i].release(); s->ev[i].release(); }
+  s->ws.release();
   cs_shamir_state_free(s->state);
   delete s;
 }
@@ -1506,20 +1369,11 @@ int cs_plonk_shamir_prove(cs_plonk_shamir* s, cs_net* net, const uint64_t* h_pub
   if (net->n != s->n_parties || net->id != s->party)
     return fail(CS_ERR_ARG, "cs_plonk_shamir_prove: the net is party %d of %d, the session is party %d of %d", net->id, net->n,
                 s->party, s->n_parties);
-  const cs_plonk_pk* pk = s->pk;
-  if (n_public_inputs != (size_t)pk->n_public + 1)
-    return fail(CS_ERR_ARG, "cs_plonk_shamir_prove: %zu public inputs, the key expects %u", n_public_inputs, pk->n_public + 1);
-  if (n_witness != (size_t)pk->n_vars - pk->n_additions - pk->n_public - 1)
-    return fail(CS_ERR_ARG, "cs_plonk_shamir_prove: %zu witness shares, the key expects %u", n_witness,
-                pk->n_vars - pk->n_additions - pk->n_public - 1);
+  CS_TRY(check_counts(s->pk, n_public_inputs, n_witness, "cs_plonk_shamir_prove"));
   CS_CUDA(cudaSetDevice(s->ctx->device));
-  switch (pk->curve) {
-    case CS_BN254: return sh_prove_t<Bn254Cfg>(s, net, h_public_inputs, h_witness_shares, h_blinder_shares, out_points, out_evals, out_blinder_shares);
-#if defined(CS_ENABLE_BLS12_381)
-    case CS_BLS12_381: return sh_prove_t<Bls381Cfg>(s, net, h_public_inputs, h_witness_shares, h_blinder_shares, out_points, out_evals, out_blinder_shares);
-#endif
-    default: return fail(CS_ERR_ARG, "unsupported curve id %d", pk->curve);
-  }
+  CS_DISPATCH_CURVE(s->pk->curve, return sh_prove_t<Cfg>(s, net, h_public_inputs, h_witness_shares, h_blinder_shares, out_points,
+                                                         out_evals, out_blinder_shares));
+  return 0;
 }
 
 size_t cs_plonk_shamir_pairs(const cs_plonk_shamir* s) { return s ? s->pairs : 0; }
@@ -1528,13 +1382,8 @@ double cs_plonk_shamir_pair_ms(const cs_plonk_shamir* s) { return s ? s->pair_ms
 
 size_t cs_plonk_shamir_device_bytes(const cs_plonk_shamir* s) {
   if (!s) return 0;
-  const DevBuf* all[] = {&s->w, &s->arena, &s->pair_t, &s->pair_2t, &s->addv, &s->pubv, &s->t, &s->tz, &s->t1, &s->t2, &s->t3,
-                         &s->tmp0, &s->tmp1, &s->totals, &s->small};
-  size_t b = shamir_state_device_bytes(s->state);
-  for (const DevBuf* x : all) b += x->cap;
-  for (int i = 0; i < 3; i++) b += s->buf[i].cap;
-  for (int i = 0; i < 4; i++) b += s->poly[i].cap + s->ev[i].cap;
-  return b;
+  return shamir_state_device_bytes(s->state) + s->ws.bytes() + s->arena.cap + s->pair_t.cap + s->pair_2t.cap + s->addv.cap +
+         s->pubv.cap;
 }
 
 }  // extern "C"

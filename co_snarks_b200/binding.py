@@ -215,6 +215,8 @@ SIGNATURES = {
     "cs_groth16_witness_map_libsnark": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "cs_groth16_prove_plain": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "cs_groth16_prove_plain_device": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
+    "cs_groth16_prove_plain_batch": (C.c_int, [C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p,
+                                               C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
     "cs_groth16_rep3_local_parts": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_uint] + [C.c_void_p] * 11),
     "cs_groth16_rep3_local_prf": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_uint] + [C.c_void_p] * 12),
     "cs_groth16_shamir_local": (C.c_int, [C.c_void_p, C.c_void_p] + [C.c_void_p] * 9),
@@ -870,6 +872,28 @@ class Groth16Key:
         self.ctx._check(self.ctx.lib.cs_groth16_prove_plain(
             self.ctx.h, self.h, _ptr(public_inputs), _ptr(witness), _ptr(r_mont), _ptr(s_mont),
             _ptr(a), _ptr(b), _ptr(c)))
+        return a, b, c
+
+    def prove_plain_batch(self, public_inputs, witness=None, r_mont=None, s_mont=None, d_witness=None):
+        """K plain proofs in one call (cs_groth16_prove_plain_batch).  public_inputs: uint64 [K, ni, 4]; witness:
+        uint64 [K, nw, 4] on the host, or d_witness: a device pointer to the same layout; r_mont, s_mont: [K, 4].
+        -> (A [K, 2 fq], B [K, 4 fq], C [K, 2 fq]) affine Montgomery limb arrays; row j equals prove_plain's
+        result for proof j."""
+        pub = np.ascontiguousarray(public_inputs, dtype=np.uint64)
+        K = pub.shape[0]
+        ni = pub.shape[1] if pub.ndim > 1 else 0
+        wit = None if witness is None else np.ascontiguousarray(witness, dtype=np.uint64)
+        nw = wit.shape[1] if wit is not None and wit.ndim > 1 else (self.nw or 0)
+        r = np.ascontiguousarray(r_mont, dtype=np.uint64)
+        s = np.ascontiguousarray(s_mont, dtype=np.uint64)
+        if r.size != 4 * K or s.size != 4 * K:
+            raise CsError("prove_plain_batch: need one r and one s per proof")
+        a = np.zeros((K, 2 * self.fq), dtype=np.uint64)
+        b = np.zeros((K, 4 * self.fq), dtype=np.uint64)
+        c = np.zeros((K, 2 * self.fq), dtype=np.uint64)
+        self.ctx._check(self.ctx.lib.cs_groth16_prove_plain_batch(
+            self.ctx.h, self.h, K, _ptr(pub), ni, _ptr(wit) if wit is not None and wit.size else None,
+            C.c_void_p(d_witness) if d_witness else None, nw, _ptr(r), _ptr(s), _ptr(a), _ptr(b), _ptr(c)))
         return a, b, c
 
     def prove_plain_device(self, public_inputs, d_witness, r_mont, s_mont):

@@ -53,7 +53,8 @@ static int ntt_smem_optin() {
 #if !defined(CS_EMU)
 #define CS_NTT_ATTR(D, S, KB) \
   CS_CUDA(cudaFuncSetAttribute(k_ntt_pass<FrP, D, S>, cudaFuncAttributeMaxDynamicSharedMemorySize, KB * 1024))
-  CS_NTT_ATTR(true, false, 64); CS_NTT_ATTR(false, false, 64); CS_NTT_ATTR(true, true, 96); CS_NTT_ATTR(false, true, 96);
+  CS_NTT_ATTR(true, false, (NTT_SMEM_PLAIN >> 10)); CS_NTT_ATTR(false, false, (NTT_SMEM_PLAIN >> 10));
+  CS_NTT_ATTR(true, true, (NTT_SMEM_TWS >> 10)); CS_NTT_ATTR(false, true, (NTT_SMEM_TWS >> 10));
 #undef CS_NTT_ATTR
 #endif
   return 0;
@@ -188,13 +189,14 @@ int cs_memcpy_d2h(cs_ctx* ctx, void* h_dst, const void* d_src, size_t bytes) {
 // ------------------------------------------------------------------------------------------- MSM
 namespace cs {
 
-int table_budget(cs_ctx* ctx, size_t* out) {
+int table_budget(cs_ctx* ctx, size_t* out, size_t reusable) {
   size_t avail = 0, total = 0;
 #if defined(CS_EMU)
   avail = total = 80ull << 30;  // the CPU emulation has no device: an 80 GB H100's, so full tables are picked as there
 #else
   CS_CUDA(cudaMemGetInfo(&avail, &total));
 #endif
+  avail += reusable;
   avail = avail > TABLE_MARGIN ? avail - TABLE_MARGIN : 0;
   *out = ctx->table_budget && ctx->table_budget < avail ? ctx->table_budget : avail;
   return 0;
@@ -261,11 +263,13 @@ int bases_upload_t(cs_ctx* ctx, const uint64_t* h_points, size_t n, int window_b
 
 template <class Cfg, int G>
 int msm_enqueue_t(cs_ctx* ctx, int slot, cudaStream_t st, const cs_bases* b, size_t offset,
-                  const uint32_t* d_scalars, unsigned sstride, size_t n, int mont, int sort_slot, bool view) {
+                  const uint32_t* d_scalars, unsigned sstride, size_t n, int mont, int sort_slot, bool view, unsigned K,
+                  size_t pstride) {
   typedef typename GroupOf<Cfg, G>::F F;
   return msm_enqueue<F, typename Cfg::FrP>(ctx->msm_ws[slot], b->table.as<Affine<F>>(), b->infmask.as<uint32_t>(), (uint32_t)b->n, b->sh,
                                            (uint32_t)offset, d_scalars, sstride, (uint32_t)n, mont, st,
-                                           sort_slot >= 0 ? &ctx->msm_ws[sort_slot] : nullptr, view, b->m260, ctx->acc[slot]);
+                                           sort_slot >= 0 ? &ctx->msm_ws[sort_slot] : nullptr, view, b->m260, ctx->acc[slot],
+                                           K, (uint32_t)pstride);
 }
 
 // After the stream has drained: XYZZ (pinned) -> affine on the host.
@@ -279,18 +283,20 @@ void msm_finish_t(cs_ctx* ctx, int slot, uint64_t* out_affine, int* out_inf) {
 }
 
 int msm_enqueue_dyn(cs_ctx* ctx, int slot, cudaStream_t st, const cs_bases* b, size_t offset,
-                    const uint32_t* d_scalars, unsigned sstride, size_t n, int mont, int sort_slot, bool view) {
+                    const uint32_t* d_scalars, unsigned sstride, size_t n, int mont, int sort_slot, bool view, unsigned K,
+                    size_t pstride) {
   CS_DISPATCH_CURVE(b->curve, {
-    if (b->group == CS_G1) return msm_enqueue_t<Cfg, 0>(ctx, slot, st, b, offset, d_scalars, sstride, n, mont, sort_slot, view);
-    return msm_enqueue_t<Cfg, 1>(ctx, slot, st, b, offset, d_scalars, sstride, n, mont, sort_slot, view);
+    if (b->group == CS_G1)
+      return msm_enqueue_t<Cfg, 0>(ctx, slot, st, b, offset, d_scalars, sstride, n, mont, sort_slot, view, K, pstride);
+    return msm_enqueue_t<Cfg, 1>(ctx, slot, st, b, offset, d_scalars, sstride, n, mont, sort_slot, view, K, pstride);
   });
   return 0;
 }
 int msm_sort_shared_dyn(cs_ctx* ctx, int slot, cudaStream_t st, const cs_bases* b, const uint32_t* d_scalars,
-                        unsigned sstride, size_t n, int mont) {
+                        unsigned sstride, size_t n, int mont, unsigned K, size_t pstride) {
   CS_DISPATCH_CURVE(b->curve, {
     return msm_sort<typename Cfg::FrP>(ctx->msm_ws[slot], nullptr, (uint32_t)n, b->sh, 0, d_scalars, sstride, (uint32_t)n,
-                                       mont, st);
+                                       mont, st, K, (uint32_t)pstride);
   });
   return 0;
 }
@@ -552,7 +558,7 @@ int domain_create_t(cs_ctx* ctx, unsigned log_n, const uint64_t* gen_mont, cs_do
 
 int ntt_run(cs_ctx* ctx, const cs_domain* d, uint32_t* d_data, unsigned batch, bool inverse_in_to_out,
             const uint32_t* d_post, cudaStream_t st) {
-  if (batch != 1 && batch != 2) return fail(CS_ERR_ARG, "ntt: batch must be 1 or 2");
+  if (batch == 0) return fail(CS_ERR_ARG, "ntt: batch must be >= 1");
   if (d->log_n == 0) return 0;
   // CS_NTT_V2=1 selects the TMA-staged radix-8 pass (cs_ntt8.cuh).  Both passes are bound by the instruction mix of a
   // butterfly (one product + add + sub), not by the copies, and the TMA pass pays a tile set-up at small sizes, so the
@@ -563,7 +569,7 @@ int ntt_run(cs_ctx* ctx, const cs_domain* d, uint32_t* d_data, unsigned batch, b
     typedef typename Cfg::FrP FrP;
     const uint32_t* twp = inverse_in_to_out ? d->tw_inv.as<uint32_t>() : d->tw_fwd.as<uint32_t>();
     const uint32_t* scale = (inverse_in_to_out && !d_post) ? d->inv_n.as<uint32_t>() : nullptr;
-    if (v2_env) {  // TMA-staged tiles + register radix-8 (cs_ntt8.cuh) from 2^12 on
+    if (v2_env && batch <= 2) {  // TMA-staged tiles + register radix-8 (cs_ntt8.cuh) from 2^12 on
       bool used = false;
       CS_TRY((ntt_enqueue8<FrP>(d_data, twp, d->log_n, batch, !inverse_in_to_out, d_post, scale, st, &used)));
       if (used) return 0;

@@ -33,6 +33,7 @@ struct cs_groth16_pk {
   int wit_src[4] = {0, 1, 2, 3};
   cs_domain* dom_ark = nullptr;
   DevBuf coset_tab_ark, ginv_pows, vinv_over_n;
+  DevBuf d_pt;  // the single-point work of a batch of proofs (batch_points)
 };
 
 namespace {
@@ -98,28 +99,33 @@ int upload(cs_ctx* ctx, DevBuf& buf, const void* src, size_t bytes) {
 
 // CircomReduction::witness_map_from_matrices on the device.  Leaves h (n half shares) in pk->d_c.
 // d_pub / d_wit must already hold the inputs; masks (Rep3) in d_m1 / d_m2 or null.
+// K > 1 (plain values only): the witness maps of K proofs at once -- public inputs [K][ni] in d_pub, witnesses [K][nw]
+// from d_wit -- with a, b, c and h as K interleaved columns ([n][K]), so that each transform is one NTT call.
 template <class Cfg>
 int witness_map_device(cs_ctx* ctx, cs_groth16_pk* pk, int kind, int party, const uint32_t* d_wit, bool have_m1,
-                       bool have_m2, cudaStream_t st) {
+                       bool have_m2, cudaStream_t st, uint32_t K = 1) {
   typedef typename Cfg::FrP FrP;
   const unsigned batch = kind == CS_REP3 ? 2 : 1;
   const int pub_comp = kind == CS_REP3 ? (party == 0 ? 0 : (party == 1 ? 1 : -1)) : 0;
   const uint32_t n = (uint32_t)pk->n;
-  CS_TRY(pk->d_a.reserve((size_t)n * batch * 32));
-  CS_TRY(pk->d_b.reserve((size_t)n * batch * 32));
-  CS_TRY(pk->d_c.reserve((size_t)n * 32));
+  if (K > 1 && kind != CS_PLAIN) return fail(CS_ERR_ARG, "witness map: batches are of plain witnesses");
+  CS_TRY(pk->d_a.reserve((size_t)n * batch * K * 32));
+  CS_TRY(pk->d_b.reserve((size_t)n * batch * K * 32));
+  CS_TRY(pk->d_c.reserve((size_t)n * K * 32));
   // a = A w (+ promoted public rows, reduction.rs:104-113), b = B w   (evaluate_constraint)
   CS_SPAN("witness map from matrices");
   {
   CS_SPAN("evaluate constraints + coset table computation");
-  CS_LAUNCH(k_spmv<FrP>, ceil_div(n, 128), 128, 0, st, pk->a_rowptr.as<uint32_t>(), pk->a_col.as<uint32_t>(),
+  const dim3 grid(ceil_div(n, 128), K);
+  const uint32_t wps = (uint32_t)pk->nw * batch;
+  CS_LAUNCH(k_spmv<FrP>, grid, 128, 0, st, pk->a_rowptr.as<uint32_t>(), pk->a_col.as<uint32_t>(),
             pk->a_coeff.as<uint32_t>(), pk->d_pub.as<uint32_t>(), (uint32_t)pk->ni, d_wit, batch, batch,
-            pub_comp, (uint32_t)pk->nc, (uint32_t)pk->ni, n, pk->d_a.as<uint32_t>());
-  CS_LAUNCH(k_spmv<FrP>, ceil_div(n, 128), 128, 0, st, pk->b_rowptr.as<uint32_t>(), pk->b_col.as<uint32_t>(),
+            pub_comp, (uint32_t)pk->nc, (uint32_t)pk->ni, n, wps, batch * K, pk->d_a.as<uint32_t>());
+  CS_LAUNCH(k_spmv<FrP>, grid, 128, 0, st, pk->b_rowptr.as<uint32_t>(), pk->b_col.as<uint32_t>(),
             pk->b_coeff.as<uint32_t>(), pk->d_pub.as<uint32_t>(), (uint32_t)pk->ni, d_wit, batch, batch,
-            pub_comp, (uint32_t)pk->nc, 0u, n, pk->d_b.as<uint32_t>());
+            pub_comp, (uint32_t)pk->nc, 0u, n, wps, batch * K, pk->d_b.as<uint32_t>());
   }
-  unsigned blocks = ceil_div(n, 256);
+  unsigned blocks = ceil_div((size_t)n * K, 256);
   if (blocks > CS_NUM_SMS * 16) blocks = CS_NUM_SMS * 16;
   // c = local_mul_vec(a, b)   (reduction.rs:160)
   CS_SPAN("c: local_mul_vec / a, b, c: distribute powers (fft/ifft)");
@@ -129,16 +135,16 @@ int witness_map_device(cs_ctx* ctx, cs_groth16_pk* pk, int kind, int party, cons
               pk->d_c.as<uint32_t>(), (size_t)n);
   else
     CS_LAUNCH(k_plain_mul_sub<FrP>, blocks, 256, 0, st, pk->d_a.as<uint32_t>(), pk->d_b.as<uint32_t>(),
-              (const uint32_t*)nullptr, pk->d_c.as<uint32_t>(), (size_t)n);
+              (const uint32_t*)nullptr, pk->d_c.as<uint32_t>(), (size_t)n * K);
   // each of a, b, c: ifft_in_to_out -> * coset table -> fft_out_to_in   (reduction.rs:135-178);
   // the table multiply and the 1/n are fused into the last iNTT pass.
   const uint32_t* post = pk->log_n ? pk->coset_tab.as<uint32_t>() : nullptr;
-  CS_TRY(ntt_run(ctx, pk->dom, pk->d_a.as<uint32_t>(), batch, true, post, st));
-  CS_TRY(ntt_run(ctx, pk->dom, pk->d_a.as<uint32_t>(), batch, false, nullptr, st));
-  CS_TRY(ntt_run(ctx, pk->dom, pk->d_b.as<uint32_t>(), batch, true, post, st));
-  CS_TRY(ntt_run(ctx, pk->dom, pk->d_b.as<uint32_t>(), batch, false, nullptr, st));
-  CS_TRY(ntt_run(ctx, pk->dom, pk->d_c.as<uint32_t>(), 1, true, post, st));
-  CS_TRY(ntt_run(ctx, pk->dom, pk->d_c.as<uint32_t>(), 1, false, nullptr, st));
+  CS_TRY(ntt_run(ctx, pk->dom, pk->d_a.as<uint32_t>(), batch * K, true, post, st));
+  CS_TRY(ntt_run(ctx, pk->dom, pk->d_a.as<uint32_t>(), batch * K, false, nullptr, st));
+  CS_TRY(ntt_run(ctx, pk->dom, pk->d_b.as<uint32_t>(), batch * K, true, post, st));
+  CS_TRY(ntt_run(ctx, pk->dom, pk->d_b.as<uint32_t>(), batch * K, false, nullptr, st));
+  CS_TRY(ntt_run(ctx, pk->dom, pk->d_c.as<uint32_t>(), K, true, post, st));
+  CS_TRY(ntt_run(ctx, pk->dom, pk->d_c.as<uint32_t>(), K, false, nullptr, st));
   // h = local_mul_vec(a', b') - c'   (reduction.rs:182-190), in place over c
   CS_SPAN("ab: local_mul_vec + compute ab");
   if (kind == CS_REP3)
@@ -147,7 +153,7 @@ int witness_map_device(cs_ctx* ctx, cs_groth16_pk* pk, int kind, int party, cons
               pk->d_c.as<uint32_t>(), (size_t)n);
   else
     CS_LAUNCH(k_plain_mul_sub<FrP>, blocks, 256, 0, st, pk->d_a.as<uint32_t>(), pk->d_b.as<uint32_t>(),
-              pk->d_c.as<uint32_t>(), pk->d_c.as<uint32_t>(), (size_t)n);
+              pk->d_c.as<uint32_t>(), pk->d_c.as<uint32_t>(), (size_t)n * K);
   CS_CUDA(cudaGetLastError());
   return 0;
 }
@@ -206,14 +212,14 @@ int witness_map_libsnark_device(cs_ctx* ctx, cs_groth16_pk* pk, int kind, int pa
   CS_TRY(pk->d_c.reserve((size_t)n * 32));
   CS_LAUNCH(k_spmv<FrP>, ceil_div(n, 128), 128, 0, st, pk->a_rowptr.as<uint32_t>(), pk->a_col.as<uint32_t>(),
             pk->a_coeff.as<uint32_t>(), pk->d_pub.as<uint32_t>(), (uint32_t)pk->ni, d_wit, batch, batch, pub_comp,
-            (uint32_t)pk->nc, (uint32_t)pk->ni, n, pk->d_a.as<uint32_t>());
+            (uint32_t)pk->nc, (uint32_t)pk->ni, n, 0u, batch, pk->d_a.as<uint32_t>());
   CS_LAUNCH(k_spmv<FrP>, ceil_div(n, 128), 128, 0, st, pk->b_rowptr.as<uint32_t>(), pk->b_col.as<uint32_t>(),
             pk->b_coeff.as<uint32_t>(), pk->d_pub.as<uint32_t>(), (uint32_t)pk->ni, d_wit, batch, batch, pub_comp,
-            (uint32_t)pk->nc, 0u, n, pk->d_b.as<uint32_t>());
+            (uint32_t)pk->nc, 0u, n, 0u, batch, pk->d_b.as<uint32_t>());
   // c from the C matrix as HALF shares (reduction.rs:292-298)
   CS_LAUNCH(k_spmv<FrP>, ceil_div(n, 128), 128, 0, st, pk->c_rowptr.as<uint32_t>(), pk->c_col.as<uint32_t>(),
             pk->c_coeff.as<uint32_t>(), pk->d_pub.as<uint32_t>(), (uint32_t)pk->ni, d_wit, 1u, batch, pub_comp_hs,
-            (uint32_t)pk->nc, 0u, n, pk->d_c.as<uint32_t>());
+            (uint32_t)pk->nc, 0u, n, 0u, 1u, pk->d_c.as<uint32_t>());
   const uint32_t* post = pk->log_n ? pk->coset_tab_ark.as<uint32_t>() : nullptr;
   CS_TRY(ntt_run(ctx, pk->dom_ark, pk->d_a.as<uint32_t>(), batch, true, post, st));
   CS_TRY(ntt_run(ctx, pk->dom_ark, pk->d_a.as<uint32_t>(), batch, false, nullptr, st));
@@ -484,6 +490,206 @@ int prove_plain_t(cs_ctx* ctx, cs_groth16_pk* pk, const uint64_t* h_pub, const u
   return 0;
 }
 
+
+// ---- batches of plain proofs: CoGroth16::prove (plain driver) applied to K witnesses of one circuit
+// A sub-batch of K proofs runs one witness map over K interleaved columns, one sort and one accumulation per MSM
+// with a proof dimension (msm_enqueue's K), and does every proof's single-point work on the device (k_point_*).
+
+// Carves the point work's device buffers for K proofs out of one allocation; null base = sizes only.
+template <class Cfg>
+struct BatchPoints {
+  typedef typename GroupOf<Cfg, 0>::F F1;
+  typedef typename GroupOf<Cfg, 1>::F F2;
+  Affine<F1> *b1, *cst1, *cb, *out_c;  // A and B1 term bases [2K][ni], their shared points [2], C's bases [K][3], C [K]
+  Affine<F2> *b2, *cst2, *out_b2;      // B2 term bases [K][ni], its shared point, B2 [K]
+  uint32_t *sc1, *sc3;                 // scalars: A and B1 terms [2K][ni] (B2's are B1's), C's terms [K][3]
+  Xyzz<F1> *prod1, *prod3, *sum1;
+  Xyzz<F2> *prod2, *sum2;
+  size_t bytes = 0;
+  BatchPoints(char* base, size_t K, size_t ni) {
+    auto take = [&](size_t n) { char* p = base ? base + bytes : nullptr; bytes += (n + 255) & ~(size_t)255; return p; };
+    b1 = (Affine<F1>*)take(2 * K * ni * sizeof(Affine<F1>));
+    cst1 = (Affine<F1>*)take(2 * sizeof(Affine<F1>));
+    cb = (Affine<F1>*)take(3 * K * sizeof(Affine<F1>));
+    out_c = (Affine<F1>*)take(K * sizeof(Affine<F1>));
+    b2 = (Affine<F2>*)take(K * ni * sizeof(Affine<F2>));
+    cst2 = (Affine<F2>*)take(sizeof(Affine<F2>));
+    out_b2 = (Affine<F2>*)take(K * sizeof(Affine<F2>));
+    sc1 = (uint32_t*)take(2 * K * ni * 32);
+    sc3 = (uint32_t*)take(3 * K * 32);
+    prod1 = (Xyzz<F1>*)take(2 * K * ni * sizeof(Xyzz<F1>));
+    prod3 = (Xyzz<F1>*)take(3 * K * sizeof(Xyzz<F1>));
+    sum1 = (Xyzz<F1>*)take(2 * K * sizeof(Xyzz<F1>));
+    prod2 = (Xyzz<F2>*)take(K * ni * sizeof(Xyzz<F2>));
+    sum2 = (Xyzz<F2>*)take(K * sizeof(Xyzz<F2>));
+  }
+};
+
+// Device bytes of the scratch of a sub-batch of K proofs: the witness-map vectors and inputs, the workspaces of the
+// shared witness sort and the five MSMs (bounded as in key_bytes) and the point work.
+template <class Cfg>
+size_t batch_bytes(const cs_groth16_pk* pk, size_t K, bool host_wit) {
+  typedef typename GroupOf<Cfg, 0>::F F1;
+  typedef typename GroupOf<Cfg, 1>::F F2;
+  const size_t n = pk->n, nw = pk->nw;
+  size_t b = 3 * DevBuf::alloc_size(n * K * 32) + DevBuf::alloc_size(pk->ni * K * 32) +
+             (host_wit ? DevBuf::alloc_size(nw * K * 32) : 0) + DevBuf::alloc_size(BatchPoints<Cfg>(nullptr, K, pk->ni).bytes);
+  if (nw) {
+    const MsmShape sw = pk->a_query->sh;
+    b += 5 * msm_sort_bytes(sw, nw, K) + 3 * msm_accum_bytes<F1>(sw, nw, K) + msm_accum_bytes<F2>(sw, nw, K);
+  }
+  const MsmShape shh = pk->h_query->sh;
+  return b + msm_sort_bytes(shh, n, K) + msm_accum_bytes<F1>(shh, n, K);
+}
+
+// Proofs per sub-batch: the most, up to K, that the MSM limits (msm_max_batch), the NTT's pass tile and the device
+// memory allow.  The memory is what the table budget leaves (table_budget) plus the scratch the key and the context
+// already hold, which a larger sub-batch reallocates.  One proof always runs: it fails where a single proof would.
+template <class Cfg>
+int pick_sub_batch(cs_ctx* ctx, cs_groth16_pk* pk, size_t K, bool host_wit, size_t* out) {
+  size_t kmax = K;
+  if (pk->nw) kmax = std::min<size_t>(kmax, msm_max_batch(pk->a_query->sh, (uint32_t)pk->nw));
+  kmax = std::min<size_t>(kmax, msm_max_batch(pk->h_query->sh, (uint32_t)pk->n));
+  if (pk->log_n)
+    while (kmax > 1 && !ntt_max_stages((uint32_t)kmax, true)) kmax--;
+  size_t held = pk->d_a.cap + pk->d_b.cap + pk->d_c.cap + pk->d_pub.cap + pk->d_wit.cap + pk->d_pt.cap, budget = 0;
+  for (int i = 0; i <= CS_NSIDE; i++) held += ctx->msm_ws[i].bytes();
+  CS_TRY(table_budget(ctx, &budget, held));
+  size_t lo = 1, hi = kmax;  // largest K' in [1, kmax] whose scratch fits, or 1
+  while (lo < hi) {
+    const size_t mid = lo + (hi - lo + 1) / 2;
+    if (batch_bytes<Cfg>(pk, mid, host_wit) <= budget) lo = mid; else hi = mid - 1;
+  }
+  *out = lo;
+  return 0;
+}
+
+template <class Cfg>
+int prove_plain_batch_t(cs_ctx* ctx, cs_groth16_pk* pk, size_t K, const uint64_t* h_pub, const uint64_t* h_wit,
+                        const uint64_t* d_wit, const uint64_t* r, const uint64_t* s, uint64_t* out_a, uint64_t* out_b,
+                        uint64_t* out_c) {
+  typedef HostGroup<Cfg, 0> H1;
+  typedef HostGroup<Cfg, 1> H2;
+  typedef host::HFp<typename Cfg::FrP> HR;
+  typedef typename GroupOf<Cfg, 0>::F F1;
+  typedef typename GroupOf<Cfg, 1>::F F2;
+  typedef typename Cfg::FrP FrP;
+  constexpr size_t G1L = 2 * H1::HF::N, G2L = 4 * H1::HF::N, FR = HR::N;
+  const size_t ni = pk->ni, nw = pk->nw;
+  CS_CUDA(cudaSetDevice(ctx->device));
+  size_t Kb = 1;
+  CS_TRY(pick_sub_batch<Cfg>(ctx, pk, K, h_wit != nullptr, &Kb));
+  CS_TRY(pk->d_pt.reserve(BatchPoints<Cfg>(nullptr, Kb, ni).bytes));
+  const BatchPoints<Cfg> bp(pk->d_pt.as<char>(), Kb, ni);
+  // the fixed points: term bases of every proof (delta and the public-input heads), the shared sums (alpha_1 +
+  // query[0], ...) and delta_1 in C's bases; the same for every sub-batch
+  {
+    std::vector<uint64_t> b1(2 * Kb * ni * G1L), b2(Kb * ni * G2L), cb(3 * Kb * G1L, 0), cst1(2 * G1L), cst2(G2L);
+    for (size_t p = 0; p < Kb; p++)
+      for (size_t j = 0; j < ni; j++) {
+        const uint64_t* a = j ? pk->a_head.data() + j * G1L : pk->delta_g1.data();
+        const uint64_t* b = j ? pk->b1_head.data() + j * G1L : pk->delta_g1.data();
+        const uint64_t* c = j ? pk->b2_head.data() + j * G2L : pk->delta_g2.data();
+        memcpy(&b1[(p * ni + j) * G1L], a, G1L * 8);
+        memcpy(&b1[((Kb + p) * ni + j) * G1L], b, G1L * 8);
+        memcpy(&b2[(p * ni + j) * G2L], c, G2L * 8);
+      }
+    for (size_t p = 0; p < Kb; p++) memcpy(&cb[(3 * p + 2) * G1L], pk->delta_g1.data(), G1L * 8);
+    H1::store(cst1.data(), host::hadd(H1::load(pk->alpha_g1.data()), H1::load(pk->a_head.data())));
+    H1::store(cst1.data() + G1L, host::hadd(H1::load(pk->beta_g1.data()), H1::load(pk->b1_head.data())));
+    H2::store(cst2.data(), host::hadd(H2::load(pk->beta_g2.data()), H2::load(pk->b2_head.data())));
+    CS_CUDA(cudaMemcpyAsync(bp.b1, b1.data(), b1.size() * 8, cudaMemcpyHostToDevice, ctx->stream));
+    CS_CUDA(cudaMemcpyAsync(bp.b2, b2.data(), b2.size() * 8, cudaMemcpyHostToDevice, ctx->stream));
+    CS_CUDA(cudaMemcpyAsync(bp.cb, cb.data(), cb.size() * 8, cudaMemcpyHostToDevice, ctx->stream));
+    CS_CUDA(cudaMemcpyAsync(bp.cst1, cst1.data(), cst1.size() * 8, cudaMemcpyHostToDevice, ctx->stream));
+    CS_CUDA(cudaMemcpyAsync(bp.cst2, cst2.data(), cst2.size() * 8, cudaMemcpyHostToDevice, ctx->stream));
+    CS_CUDA(cudaStreamSynchronize(ctx->stream));
+  }
+  std::vector<uint64_t> sc1(2 * Kb * ni * FR), sc3(3 * Kb * FR), cb(3 * Kb * G1L), ob2(Kb * G2L), oc(Kb * G1L);
+  for (size_t j0 = 0; j0 < K; j0 += Kb) {
+    const size_t k = std::min(Kb, K - j0);
+    const uint32_t kk = (uint32_t)k;
+    // scalars of the point work: A [r, pub[1..]], B1 and B2 [s, pub[1..]], C [s, r, -(r s)]
+    for (size_t p = 0; p < k; p++) {
+      const uint64_t *rp = r + (j0 + p) * FR, *sp = s + (j0 + p) * FR, *pub = h_pub + (j0 + p) * ni * FR;
+      memcpy(&sc1[p * ni * FR], rp, FR * 8);
+      memcpy(&sc1[(k + p) * ni * FR], sp, FR * 8);
+      for (size_t j = 1; j < ni; j++) {
+        memcpy(&sc1[(p * ni + j) * FR], pub + j * FR, FR * 8);
+        memcpy(&sc1[((k + p) * ni + j) * FR], pub + j * FR, FR * 8);
+      }
+      HR rr, ss;
+      memcpy(rr.l, rp, sizeof(rr.l));
+      memcpy(ss.l, sp, sizeof(ss.l));
+      const HR nrs = HR::zero() - rr * ss;
+      memcpy(&sc3[3 * p * FR], sp, FR * 8);
+      memcpy(&sc3[(3 * p + 1) * FR], rp, FR * 8);
+      memcpy(&sc3[(3 * p + 2) * FR], nrs.l, FR * 8);
+    }
+    // inputs: public [k][ni] always from the host, the witness [k][nw] from the host or in place
+    CS_TRY(upload(ctx, pk->d_pub, h_pub + j0 * ni * FR, k * ni * 32));
+    const uint32_t* wit = d_wit ? reinterpret_cast<const uint32_t*>(d_wit + j0 * nw * FR) : nullptr;
+    if (h_wit) {
+      CS_TRY(upload(ctx, pk->d_wit, h_wit + j0 * nw * FR, k * nw * 32));
+      wit = pk->d_wit.as<uint32_t>();
+    }
+    CS_CUDA(cudaMemcpyAsync(bp.sc1, sc1.data(), 2 * k * ni * 32, cudaMemcpyHostToDevice, ctx->stream));
+    CS_CUDA(cudaMemcpyAsync(bp.sc3, sc3.data(), 3 * k * 32, cudaMemcpyHostToDevice, ctx->stream));
+    // the MSMs, laid out on the streams as in local_phase: witness map -> H first, on the highest-priority stream
+    CS_TRY(ctx_fork(ctx, 5));
+    cudaStream_t wm = ctx->wm;
+    CS_CUDA(cudaStreamWaitEvent(wm, ctx->ev_fork, 0));
+    CS_TRY((witness_map_device<Cfg>(ctx, pk, CS_PLAIN, 0, wit, false, false, wm, kk)));
+    CS_TRY(msm_enqueue_dyn(ctx, 4, wm, pk->h_query, 0, pk->d_c.as<uint32_t>(), kk, pk->n, 1, -1, false, kk, 1));
+    if (nw) {
+      const cs_bases* q[4] = {pk->a_query, pk->b_g1, pk->b_g2, pk->l_query};
+      const size_t off[4] = {ni, ni, ni, 0};
+      CS_TRY(msm_sort_shared_dyn(ctx, CS_WIT_SORT, ctx->side[4], pk->a_query, wit, 1, nw, 1, kk, nw));
+      for (int j = 0; j < 4; j++) {
+        const int src = pk->wit_src[j];
+        CS_TRY(msm_enqueue_dyn(ctx, j, ctx->side[j], q[j], off[j], wit, 1, nw, 1, src < 0 || src == j ? CS_WIT_SORT : src,
+                               src == j, kk, nw));
+      }
+    }
+    CS_TRY(ctx_join(ctx, 5));
+    CS_CUDA(cudaEventRecord(ctx->ev_wm, wm));
+    CS_CUDA(cudaStreamWaitEvent(ctx->stream, ctx->ev_wm, 0));
+    // the point work (groth16.rs:232-322 with the plain driver), after the MSMs:
+    //   A = alpha_1 + query[0] + sum_j pub_j query[j] + r delta_1 + msm_A      (B1, B2 alike with s)
+    //   C = s A + r B1 - (r s) delta_1 + L + H
+    cudaStream_t st = ctx->stream;
+    auto res1 = [&](int slot) { return nw || slot == 4 ? ctx->msm_ws[slot].result.template as<Xyzz<F1>>() : nullptr; };
+    const Xyzz<F2>* res_b2 = nw ? ctx->msm_ws[2].result.as<Xyzz<F2>>() : nullptr;
+    const uint32_t T = (uint32_t)ni, nt = kk * T;
+    const uint32_t* sc_b = bp.sc1 + (size_t)nt * FrP::N;  // B1's and B2's scalars
+    CS_LAUNCH((k_point_terms<F1, FrP>), ceil_div(nt, 128), 128, 0, st, bp.b1, bp.sc1, nt, bp.prod1);
+    CS_LAUNCH((k_point_terms<F1, FrP>), ceil_div(nt, 128), 128, 0, st, bp.b1 + Kb * ni, sc_b, nt, bp.prod1 + nt);
+    CS_LAUNCH((k_point_terms<F2, FrP>), ceil_div(nt, 128), 128, 0, st, bp.b2, sc_b, nt, bp.prod2);
+    CS_LAUNCH(k_point_sum<F1>, ceil_div(kk, 128), 128, 0, st, bp.prod1, T, kk, res1(0), (const Xyzz<F1>*)nullptr, bp.cst1,
+              bp.sum1);
+    CS_LAUNCH(k_point_sum<F1>, ceil_div(kk, 128), 128, 0, st, bp.prod1 + nt, T, kk, res1(1),
+              (const Xyzz<F1>*)nullptr, bp.cst1 + 1, bp.sum1 + kk);
+    CS_LAUNCH(k_point_sum<F2>, ceil_div(kk, 128), 128, 0, st, bp.prod2, T, kk, res_b2, (const Xyzz<F2>*)nullptr, bp.cst2,
+              bp.sum2);
+    const uint32_t runs = ceil_div(kk, POINT_INV_RUN);
+    CS_LAUNCH(k_point_affine<F1>, ceil_div(runs, 128), 128, 0, st, bp.sum1, kk, 3u, bp.cb);
+    CS_LAUNCH(k_point_affine<F1>, ceil_div(runs, 128), 128, 0, st, bp.sum1 + kk, kk, 3u, bp.cb + 1);
+    CS_LAUNCH(k_point_affine<F2>, ceil_div(runs, 128), 128, 0, st, bp.sum2, kk, 1u, bp.out_b2);
+    CS_LAUNCH((k_point_terms<F1, FrP>), ceil_div(3 * kk, 128), 128, 0, st, bp.cb, bp.sc3, 3 * kk, bp.prod3);
+    CS_LAUNCH(k_point_sum<F1>, ceil_div(kk, 128), 128, 0, st, bp.prod3, 3u, kk, res1(3), res1(4), (const Affine<F1>*)nullptr,
+              bp.sum1);
+    CS_LAUNCH(k_point_affine<F1>, ceil_div(runs, 128), 128, 0, st, bp.sum1, kk, 1u, bp.out_c);
+    CS_CUDA(cudaGetLastError());
+    CS_CUDA(cudaMemcpyAsync(cb.data(), bp.cb, 3 * k * G1L * 8, cudaMemcpyDeviceToHost, st));
+    CS_CUDA(cudaMemcpyAsync(ob2.data(), bp.out_b2, k * G2L * 8, cudaMemcpyDeviceToHost, st));
+    CS_CUDA(cudaMemcpyAsync(oc.data(), bp.out_c, k * G1L * 8, cudaMemcpyDeviceToHost, st));
+    CS_CUDA(cudaStreamSynchronize(st));
+    for (size_t p = 0; p < k; p++) memcpy(out_a + (j0 + p) * G1L, &cb[3 * p * G1L], G1L * 8);
+    memcpy(out_b + j0 * G2L, ob2.data(), k * G2L * 8);
+    memcpy(out_c + j0 * G1L, oc.data(), k * G1L * 8);
+  }
+  return 0;
+}
 
 // Rep3CoGroth16::prove for one party (groth16.rs:360-379, prove_inner :125-177, create_proof_with_assignment
 // :207-338 with Rep3Groth16Driver, mpc/rep3.rs).  role: 0 = the whole party on one GPU, 1 = the party's
@@ -791,7 +997,8 @@ void cs_groth16_pk_free(cs_groth16_pk* pk) {
   if (!pk) return;
   DevBuf* bufs[] = {&pk->a_rowptr, &pk->a_col, &pk->a_coeff, &pk->b_rowptr, &pk->b_col, &pk->b_coeff, &pk->coset_tab,
                     &pk->d_pub, &pk->d_wit, &pk->d_a, &pk->d_b, &pk->d_c, &pk->d_m1, &pk->d_m2,
-                    &pk->c_rowptr, &pk->c_col, &pk->c_coeff, &pk->coset_tab_ark, &pk->ginv_pows, &pk->vinv_over_n};
+                    &pk->c_rowptr, &pk->c_col, &pk->c_coeff, &pk->coset_tab_ark, &pk->ginv_pows, &pk->vinv_over_n,
+                    &pk->d_pt};
   for (DevBuf* b : bufs) b->release();
   cs_bases_free(pk->a_query);
   cs_bases_free(pk->b_g1);
@@ -890,6 +1097,25 @@ int cs_groth16_prove_plain_device(cs_ctx* ctx, cs_groth16_pk* pk, const uint64_t
 #endif
     default: return fail(CS_ERR_ARG, "unsupported curve");
   }
+}
+
+int cs_groth16_prove_plain_batch(cs_ctx* ctx, cs_groth16_pk* pk, size_t num_proofs, const uint64_t* h_public_inputs,
+                                 size_t num_public, const uint64_t* h_witness, const uint64_t* d_witness, size_t num_witness,
+                                 const uint64_t* h_r_mont, const uint64_t* h_s_mont, uint64_t* out_a, uint64_t* out_b,
+                                 uint64_t* out_c) {
+  if (!ctx || !pk || !h_public_inputs || !h_r_mont || !h_s_mont || !out_a || !out_b || !out_c)
+    return fail(CS_ERR_ARG, "cs_groth16_prove_plain_batch: NULL argument");
+  if (num_proofs == 0) return fail(CS_ERR_ARG, "cs_groth16_prove_plain_batch: a batch needs at least one proof");
+  if (num_public != pk->ni || num_witness != pk->nw)
+    return fail(CS_ERR_ARG, "cs_groth16_prove_plain_batch: the key takes %zu public inputs (incl. the leading one) and %zu "
+                "witness values per proof, got %zu and %zu", pk->ni, pk->nw, num_public, num_witness);
+  if (pk->nw && !h_witness == !d_witness)
+    return fail(CS_ERR_ARG, "cs_groth16_prove_plain_batch: pass the witnesses either on the host or on the device");
+  CS_DISPATCH_CURVE(pk->curve, {
+    return prove_plain_batch_t<Cfg>(ctx, pk, num_proofs, h_public_inputs, h_witness, d_witness, h_r_mont, h_s_mont, out_a,
+                                    out_b, out_c);
+  });
+  return 0;
 }
 
 // ShamirGroth16Driver's local computation is the plain driver's, applied to degree-t shares

@@ -111,12 +111,15 @@ std::atomic<uint64_t>& launch_counter();
 int ctx_fork(cs_ctx* ctx, int nside);
 int ctx_join(cs_ctx* ctx, int nside);
 // sort_slot >= 0: the MSM reads the sort last enqueued in that workspace slot over the same scalars -- as it is, or
-// (view) through a filtered view of the shared witness sort; see msm_enqueue
+// (view) through a filtered view of the shared witness sort; see msm_enqueue.  K > 1: a batch of K MSMs, proof p's
+// scalar i at (i sstride + p pstride) elements; K results in the workspace.
 int msm_enqueue_dyn(cs_ctx* ctx, int slot, cudaStream_t st, const cs_bases* b, size_t offset,
-                    const uint32_t* d_scalars, unsigned sstride, size_t n, int mont, int sort_slot = -1, bool view = false);
-// Sort of n scalars into workspace `slot` without an infinity mask, entries w * n + i, in the window shape of b
+                    const uint32_t* d_scalars, unsigned sstride, size_t n, int mont, int sort_slot = -1, bool view = false,
+                    unsigned K = 1, size_t pstride = 0);
+// Sort of n scalars (K vectors of them) into workspace `slot` without an infinity mask, entries w * n + i, in the
+// window shape of b
 int msm_sort_shared_dyn(cs_ctx* ctx, int slot, cudaStream_t st, const cs_bases* b, const uint32_t* d_scalars,
-                        unsigned sstride, size_t n, int mont);
+                        unsigned sstride, size_t n, int mont, unsigned K = 1, size_t pstride = 0);
 int msm_finish_dyn(cs_ctx* ctx, int slot, const cs_bases* b, uint64_t* out_affine, int* out_inf);
 
 // widest window an MSM can run: msm_scan takes 2^20 bucket slots, 2^(c-1) buckets plus bucket 0
@@ -127,7 +130,8 @@ static_assert((1u << (MSM_MAX_WINDOW - 1)) + 1 <= MSM_SCAN_MAX_BLOCKS * MSM_SCAN
 // budget: what cudaMemGetInfo reports free less TABLE_MARGIN (the CUDA runtime's own allocations), capped by
 // cs_ctx_set_table_budget.  k = 1 (full tables) whenever they fit.
 constexpr size_t TABLE_MARGIN = 256ull << 20;
-int table_budget(cs_ctx* ctx, size_t* out);
+// reusable: bytes the caller holds and would free before allocating (a batch's scratch as it grows)
+int table_budget(cs_ctx* ctx, size_t* out, size_t reusable = 0);
 // smallest k in 1..W with need(k) <= budget, or CS_ERR_LIMIT stating the bytes needed at k = W and the budget
 int pick_table_rows(cs_ctx* ctx, unsigned c, unsigned W, const std::function<size_t(unsigned)>& need, const char* who,
                     unsigned* k_out);

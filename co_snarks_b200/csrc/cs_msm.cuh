@@ -84,9 +84,12 @@ CS_D bool msm_base_inf(const uint32_t* __restrict__ infmask, uint32_t k) {
 //  * k_msm_bin_scatter: the block recodes its tile again and places every entry at start[b] + its row's prefix + a
 //    rank from a shared-memory cursor.
 // A histogram covers MSM_BIN_SPAN buckets (128 KB); wider windows split the buckets over grid.y, and each block
-// re-reads its tile for its share of the buckets.  The scatter takes MSM_SCATTER_SPAN buckets per grid.y slice even
-// at c = 16: its scattered 4-byte stores, not the recoding, bound it, and with a quarter of the buckets at a time the
-// output lines being written stay fewer (measured at 2^20 scalars on the H100: 412 us in four slices against 509 us
+// re-reads its tile for its share of the buckets.
+// K scalar vectors over one base set (a batch of K proofs; proof p's scalars start pstride elements after proof
+// p - 1's) sort as one: bucket (p k + g) B + d.  Each tile belongs to one proof (blocks [p nblk_p, (p + 1) nblk_p)), so
+// its table row covers only that proof's k B buckets, and the table is K times one MSM's.
+// The scatter takes MSM_SCATTER_SPAN buckets per grid.y slice even at c = 16: its scattered 4-byte stores, not the
+// recoding, bound it, and with a quarter of the buckets at a time the output lines being written stay fewer (measured at 2^20 scalars on the H100: 412 us in four slices against 509 us
 // in one, although each slice recodes the tile again).
 constexpr unsigned MSM_BIN_T = 1024;             // threads per block of k_msm_bin_count / k_msm_bin_scatter
 constexpr unsigned MSM_BIN_TILE = 4096;          // scalars per block, unless the count table would outgrow W n words
@@ -97,14 +100,17 @@ template <class FrP>
 CS_GLOBAL void __launch_bounds__(MSM_BIN_T) k_msm_bin_count(const uint32_t* __restrict__ scalars, uint32_t sstride,
                                                             uint32_t n, int mont, uint32_t c, uint32_t W, uint32_t kw,
                                                             const uint32_t* __restrict__ infmask, uint32_t offset,
-                                                            uint32_t tile, uint32_t B, uint32_t* __restrict__ tab) {
+                                                            uint32_t tile, uint32_t nblk_p, uint32_t pstride, uint32_t B,
+                                                            uint32_t* __restrict__ tab) {
   CS_DYN_SMEM(uint32_t, h);
+  const uint32_t bt = blockIdx.x % nblk_p;  // tile within proof blockIdx.x / nblk_p
+  scalars += (size_t)(blockIdx.x / nblk_p) * pstride * FrP::N;
   const uint32_t lo = blockIdx.y * MSM_BIN_SPAN + 1;  // buckets [lo, lo + span)
   const uint32_t span = B + 1 - lo < MSM_BIN_SPAN ? B + 1 - lo : MSM_BIN_SPAN;
   for (uint32_t k = threadIdx.x; k < span; k += blockDim.x) h[k] = 0;
   __syncthreads();
-  const uint32_t i1 = (blockIdx.x + 1) * tile < n ? (blockIdx.x + 1) * tile : n;
-  for (uint32_t i = blockIdx.x * tile + threadIdx.x; i < i1; i += blockDim.x) {
+  const uint32_t i1 = (bt + 1) * tile < n ? (bt + 1) * tile : n;
+  for (uint32_t i = bt * tile + threadIdx.x; i < i1; i += blockDim.x) {
     if (msm_base_inf(infmask, offset + i)) continue;
     msm_recode<FrP>(scalars, sstride, i, mont, c, W, kw, [&](uint32_t, uint32_t d) {
       const uint32_t k = (d & ~MSM_SIGN) - lo;  // wraps past span for bucket 0 and for buckets below lo
@@ -116,13 +122,15 @@ CS_GLOBAL void __launch_bounds__(MSM_BIN_T) k_msm_bin_count(const uint32_t* __re
   for (uint32_t k = threadIdx.x; k < span; k += blockDim.x) row[k] = h[k];
 }
 
-// One thread per bucket, down the nblk rows of its column; count[0] = 0 (zero digits are dropped).
+// One thread per bucket, down the nblk rows of its proof's table (B buckets per proof, NB in all); count[0] = 0 (zero
+// digits are dropped).
 constexpr unsigned MSM_BIN_SCAN_U = 16;  // rows loaded before any is rewritten: loads in flight per thread
-static CS_GLOBAL void k_msm_bin_scan(uint32_t* __restrict__ tab, uint32_t nblk, uint32_t B, uint32_t* __restrict__ count) {
+static CS_GLOBAL void k_msm_bin_scan(uint32_t* __restrict__ tab, uint32_t nblk, uint32_t B, uint32_t NB,
+                                     uint32_t* __restrict__ count) {
   const uint32_t b = blockIdx.x * blockDim.x + threadIdx.x;
   if (b == 0) count[0] = 0;
-  if (b >= B) return;
-  uint32_t* col = tab + b;
+  if (b >= NB) return;
+  uint32_t* col = tab + (size_t)(b / B) * nblk * B + b % B;
   uint32_t run = 0, r = 0;
   for (; r + MSM_BIN_SCAN_U <= nblk; r += MSM_BIN_SCAN_U) {
     uint32_t v[MSM_BIN_SCAN_U];
@@ -147,18 +155,21 @@ template <class FrP>
 CS_GLOBAL void __launch_bounds__(MSM_BIN_T) k_msm_bin_scatter(const uint32_t* __restrict__ scalars, uint32_t sstride,
                                                               uint32_t n, int mont, uint32_t c, uint32_t W, uint32_t kw,
                                                               const uint32_t* __restrict__ infmask, uint32_t offset,
-                                                              uint32_t tile, uint32_t B, uint32_t nbases,
+                                                              uint32_t tile, uint32_t nblk_p, uint32_t pstride,
+                                                              uint32_t B, uint32_t nbases,
                                                               const uint32_t* __restrict__ tab,
                                                               const uint32_t* __restrict__ start,
                                                               uint32_t* __restrict__ sorted) {
   CS_DYN_SMEM(uint32_t, cur);
+  const uint32_t p = blockIdx.x / nblk_p, bt = blockIdx.x % nblk_p;
+  scalars += (size_t)p * pstride * FrP::N;
   const uint32_t lo = blockIdx.y * MSM_SCATTER_SPAN + 1;
   const uint32_t span = B + 1 - lo < MSM_SCATTER_SPAN ? B + 1 - lo : MSM_SCATTER_SPAN;
   const uint32_t* row = tab + (size_t)blockIdx.x * B + (lo - 1);
-  for (uint32_t k = threadIdx.x; k < span; k += blockDim.x) cur[k] = start[lo + k] + row[k];
+  for (uint32_t k = threadIdx.x; k < span; k += blockDim.x) cur[k] = start[p * B + lo + k] + row[k];
   __syncthreads();
-  const uint32_t i1 = (blockIdx.x + 1) * tile < n ? (blockIdx.x + 1) * tile : n;
-  for (uint32_t i = blockIdx.x * tile + threadIdx.x; i < i1; i += blockDim.x) {
+  const uint32_t i1 = (bt + 1) * tile < n ? (bt + 1) * tile : n;
+  for (uint32_t i = bt * tile + threadIdx.x; i < i1; i += blockDim.x) {
     if (msm_base_inf(infmask, offset + i)) continue;
     msm_recode<FrP>(scalars, sstride, i, mont, c, W, kw, [&](uint32_t row, uint32_t d) {
       const uint32_t k = (d & ~MSM_SIGN) - lo;
@@ -680,6 +691,19 @@ CS_GLOBAL void __launch_bounds__(128) k_msm_precompute(Affine<F>* __restrict__ t
   }
 }
 
+// --------------------------------------------------------------------------- scalar multiplication
+// s P by double-and-add over the bits of s (canonical, not Montgomery), one thread.  p may be a register copy or a
+// point in memory, which is then read at each addition (fewer registers held: what the G2 point terms need)
+template <class F, class FrP>
+CS_D Xyzz<F> scalar_mul(const Affine<F>& p, const Fp<FrP>& s) {
+  Xyzz<F> acc = Xyzz<F>::inf();
+  for (int bit = FrP::N * 32 - 1; bit >= 0; bit--) {
+    acc = dbl_xyzz(acc);
+    if ((s.l[bit >> 5] >> (bit & 31)) & 1) madd(acc, p, false);
+  }
+  return acc;
+}
+
 // --------------------------------------------------------------------------- fixed-base batch mul
 // out[i] = scalars[i] * base  (affine).  Used to synthesise proving keys / SRS (a trusted setup is n
 // fixed-base multiplications); off the per-proof path.
@@ -697,16 +721,69 @@ CS_GLOBAL void __launch_bounds__(128) k_fixed_base_mul(const Affine<F>* __restri
     s.l[4 * k] = v.x; s.l[4 * k + 1] = v.y; s.l[4 * k + 2] = v.z; s.l[4 * k + 3] = v.w;
   }
   if (mont) s = s.from_mont();
-  uint32_t lim[FrP::N];
+  const Affine<F> b = base[0];
+  out[i] = to_affine(scalar_mul<F, FrP>(b, s));
+}
+
+// --------------------------------------------------------------------------- small point linear combinations
+// out[o] = sum_j s_oj P_oj (+ per-output XYZZ addends, + one shared point) for a batch of outputs with a few terms each:
+// the single-point work of a batch of proofs (r delta_1, s A, the public-input terms, ...).  Three launches:
+//  * k_point_terms: one thread per term, prod[t] = s_t P_t by double-and-add over the bits of the (Montgomery) scalar;
+//  * k_point_sum: one thread per output, the sum of its T products, its addends and `shared`;
+//  * k_point_affine: Montgomery's trick over runs of POINT_INV_RUN outputs, one field inversion per run.
+constexpr uint32_t POINT_INV_RUN = 32;
+
+template <class F, class FrP>
+CS_GLOBAL void __launch_bounds__(128) k_point_terms(const Affine<F>* __restrict__ base, const uint32_t* __restrict__ scalars,
+                                                    uint32_t nterms, Xyzz<F>* __restrict__ prod) {
+  const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= nterms) return;
+  Fp<FrP> s;
   CS_UNROLL
-  for (int k = 0; k < FrP::N; k++) lim[k] = s.l[k];
-  Affine<F> b = base[0];
-  Xyzz<F> acc = Xyzz<F>::inf();
-  for (int bit = FrP::N * 32 - 1; bit >= 0; bit--) {
-    acc = dbl_xyzz(acc);
-    if ((lim[bit >> 5] >> (bit & 31)) & 1) madd(acc, b, false);
+  for (int k = 0; k < FrP::N; k++) s.l[k] = scalars[(size_t)t * FrP::N + k];
+  prod[t] = scalar_mul<F, FrP>(base[t], s.from_mont());
+}
+
+template <class F>
+CS_GLOBAL void __launch_bounds__(128) k_point_sum(const Xyzz<F>* __restrict__ prod, uint32_t T, uint32_t nout,
+                                                  const Xyzz<F>* __restrict__ add0, const Xyzz<F>* __restrict__ add1,
+                                                  const Affine<F>* __restrict__ shared, Xyzz<F>* __restrict__ out) {
+  const uint32_t o = blockIdx.x * blockDim.x + threadIdx.x;
+  if (o >= nout) return;
+  Xyzz<F> acc = shared ? Xyzz<F>::from_affine(*shared) : Xyzz<F>::inf();
+  for (uint32_t j = 0; j < T + 2; j++) {  // one call site of padd: a G2 addition inlined three times spills more
+    const Xyzz<F>* q = j < T ? prod + (size_t)o * T + j : (j == T ? add0 : add1);
+    if (q && j >= T) q += o;
+    if (q) padd(acc, *q);
   }
-  out[i] = to_affine(acc);
+  out[o] = acc;
+}
+
+// out[o ostride] = affine(in[o]).  The running products of the ZZZ coordinates are kept in the outputs' x until the
+// backward pass overwrites them; points at infinity are skipped by the products and come out as (0, 0).
+template <class F>
+CS_GLOBAL void __launch_bounds__(128) k_point_affine(const Xyzz<F>* __restrict__ in, uint32_t nout, uint32_t ostride,
+                                                     Affine<F>* __restrict__ out) {
+  const uint32_t lo = (blockIdx.x * blockDim.x + threadIdx.x) * POINT_INV_RUN;
+  if (lo >= nout) return;
+  const uint32_t hi = lo + POINT_INV_RUN < nout ? lo + POINT_INV_RUN : nout;
+  F run = F::one();
+  for (uint32_t o = lo; o < hi; o++) {
+    if (!in[o].is_inf()) run = run * in[o].zzz;
+    out[(size_t)o * ostride].x = run;
+  }
+  F inv = run.inverse();  // 1 / (product of every finite ZZZ of the run)
+  for (uint32_t o = hi; o-- > lo;) {  // the coordinates are loaded where they are used: no point held in registers
+    Affine<F> a = Affine<F>::inf();
+    if (!in[o].is_inf()) {
+      const F zi = o > lo ? inv * out[(size_t)(o - 1) * ostride].x : inv;  // 1 / ZZZ_o
+      inv = inv * in[o].zzz;
+      const F zzi = (zi * in[o].zz).sqr();  // (ZZ / ZZZ)^2 = 1 / ZZ
+      a.x = in[o].x * zzi;
+      a.y = in[o].y * zi;
+    }
+    out[(size_t)o * ostride] = a;
+  }
 }
 
 // --------------------------------------------------------------------------- host driver
@@ -765,6 +842,10 @@ struct MsmWorkspace {
   cudaEvent_t sorted_ev = nullptr;  // recorded once the sorted entries / slice order of this MSM are final
   bool sorted_ev_made = false, sorted_once = false;
   cudaEvent_t acc_in = nullptr, acc_out = nullptr;  // hand-off to / from the accumulation stream (msm_enqueue's st_acc)
+  size_t bytes() const {
+    return dig.cap + sorted.cap + meta.cap + part0.cap + part1.cap + part2.cap + bucket.cap + red.cap + scal.cap +
+           result.cap + order.cap;
+  }
   int mark(int i, cudaStream_t st) {
     if (!profile) return 0;
     if (!ev[i]) CS_CUDA(cudaEventCreateWithFlags(&ev[i], 0));
@@ -796,13 +877,14 @@ int msm_accum0_f52(const Affine<F>* table, const uint32_t* sorted, const uint32_
                    const uint32_t* sstart0, uint32_t nb1, uint32_t S, const uint32_t* order, const uint32_t* order_b,
                    Xyzz<F>* part0, uint32_t max_s0, cudaStream_t st);
 
-// Buffer sizes of one MSM over n scalars (W n entries) and the layout of its sort buffers.
+// Buffer sizes of K MSMs over n scalars each (K W n entries, K k B buckets) and the layout of their sort buffers.
 struct MsmSizes {
-  uint32_t nb1, S, ob;
+  uint32_t nb1, S, ob, K;
   size_t nent, max_s0, max_s1, max_s2;
-  MsmSizes(const MsmShape& sh, uint32_t n) {
-    nb1 = sh.nb() + 1;
-    nent = (size_t)sh.W * n;
+  MsmSizes(const MsmShape& sh, uint32_t n, uint32_t K_ = 1) {
+    K = K_;
+    nb1 = K * sh.nb() + 1;
+    nent = (size_t)K * sh.W * n;
     S = msm_slice(sh);
     max_s0 = nent / S + nb1;
     max_s1 = max_s0 / S + nb1;
@@ -836,10 +918,22 @@ struct MsmSortBufs {
   }
 };
 
-static inline int msm_check_limits(const MsmShape& sh, uint32_t n, uint32_t nbases) {
-  const size_t nent = (size_t)sh.W * n;
+// Largest batch of MSMs one sort and accumulation can take in shape sh: K k B + 1 bucket slots for the scan, K W n < 2^31
+// entries, K k bucket groups over k_msm_final_sum's grid.y
+static inline uint32_t msm_max_batch(const MsmShape& sh, uint32_t n) {
+  size_t K = ((size_t)MSM_SCAN_MAX_BLOCKS * MSM_SCAN_T - 1) / sh.nb();
+  if (n) K = K < ((1ull << 31) - 1) / ((size_t)sh.W * n) ? K : ((1ull << 31) - 1) / ((size_t)sh.W * n);
+  K = K < 65535 / sh.k ? K : 65535 / sh.k;
+  return (uint32_t)K;
+}
+
+static inline int msm_check_limits(const MsmShape& sh, uint32_t n, uint32_t nbases, uint32_t K = 1) {
+  const size_t nent = (size_t)K * sh.W * n;
   if (nent >= (1ull << 31) || (size_t)sh.T * nbases >= (1ull << 31))
-    return fail(-3, "msm: W*n = %zu entries or T*nbases = %zu table slots exceed 2^31", nent, (size_t)sh.T * nbases);
+    return fail(-3, "msm: K*W*n = %zu entries or T*nbases = %zu table slots exceed 2^31", nent, (size_t)sh.T * nbases);
+  if (K > 1 && K > msm_max_batch(sh, n))
+    return fail(-3, "msm: a batch of %u MSMs exceeds the %u that one sort takes in this window shape (K*k*B + 1 <= 2^20 "
+                    "buckets, K*k <= 65535 groups)", K, msm_max_batch(sh, n));
   return 0;
 }
 
@@ -884,7 +978,8 @@ int msm_smem_optin() {
 // Scalars per block of the bucket sort: MSM_BIN_TILE, or more where nblk rows of B counts would exceed the W n words
 // the table has (windows above 16 at small n).  The table then takes at most max(W n, B) words.
 static inline uint32_t msm_bin_tile(const MsmShape& sh, const MsmSizes& z, uint32_t n) {
-  const size_t rows = z.nent / sh.nb() > 1 ? z.nent / sh.nb() : 1;
+  const size_t ent = z.nent / z.K;  // entries of one MSM of the batch
+  const size_t rows = ent / sh.nb() > 1 ? ent / sh.nb() : 1;
   const size_t nblk = ceil_div(n, MSM_BIN_TILE) < rows ? ceil_div(n, MSM_BIN_TILE) : rows;
   return n ? ceil_div(n, nblk) : 1;
 }
@@ -892,7 +987,7 @@ static inline uint32_t msm_bin_tile(const MsmShape& sh, const MsmSizes& z, uint3
 // Words of ws.dig: msm_sort's per-block count table (or W n words, whichever is larger) and msm_view's keep bitmap
 // and block counts
 static inline size_t msm_sort_dig_words(const MsmShape& sh, const MsmSizes& z, uint32_t n) {
-  const size_t tab_words = (size_t)(n ? ceil_div(n, msm_bin_tile(sh, z, n)) : 0) * sh.nb();
+  const size_t tab_words = (size_t)z.K * (n ? ceil_div(n, msm_bin_tile(sh, z, n)) : 0) * sh.nb();
   return tab_words > z.nent ? tab_words : z.nent;
 }
 static inline size_t msm_view_dig_words(const MsmSizes& z) {
@@ -902,46 +997,51 @@ static inline size_t msm_view_dig_words(const MsmSizes& z) {
 
 // Bucket reduction tail of msm_enqueue: segments of L buckets (L divides B), then k_msm_final_sum over each group's
 // nseg_g segment sums in fs_blocks blocks; red holds the segment sums, the block sums and, for k > 1, the group sums.
+// A batch of K MSMs has K k groups, proof p's being [p k, (p + 1) k).
 template <class F>
 struct MsmReduce {
-  uint32_t L, nseg_g, nseg, fs_threads, fs_blocks;
+  uint32_t L, nseg_g, nseg, ngroups, fs_threads, fs_blocks;
   size_t red_elems;
-  explicit MsmReduce(const MsmShape& sh) {
+  explicit MsmReduce(const MsmShape& sh, uint32_t K = 1) {
     L = sh.B < MSM_RED_SEG ? sh.B : MSM_RED_SEG;
     nseg_g = sh.B / L;
-    nseg = sh.k * nseg_g;
+    ngroups = K * sh.k;
+    nseg = ngroups * nseg_g;
     fs_threads = sizeof(Xyzz<F>) > 128 ? 128 : 256;  // <= 32 KB of dynamic shared memory
     fs_blocks = nseg_g > 4 * fs_threads ? (nseg_g + fs_threads - 1) / fs_threads : 1;
-    red_elems = (size_t)nseg + (size_t)sh.k * fs_blocks + (sh.k > 1 ? sh.k : 0);
+    red_elems = (size_t)nseg + (size_t)ngroups * fs_blocks + (sh.k > 1 ? ngroups : 0);
   }
 };
 
-// Device bytes msm_sort / msm_view (sort) and msm_enqueue (accumulation) reserve in a workspace for n scalars
-static inline size_t msm_sort_bytes(const MsmShape& sh, uint32_t n) {
-  const MsmSizes z(sh, n);
+// Device bytes msm_sort / msm_view (sort) and msm_enqueue (accumulation) reserve in a workspace for K MSMs of n scalars
+static inline size_t msm_sort_bytes(const MsmShape& sh, uint32_t n, uint32_t K = 1) {
+  const MsmSizes z(sh, n, K);
   const size_t dig = msm_sort_dig_words(sh, z, n) > msm_view_dig_words(z) ? msm_sort_dig_words(sh, z, n) : msm_view_dig_words(z);
   return DevBuf::alloc_size(dig * 4) + DevBuf::alloc_size(z.nent * 4) + DevBuf::alloc_size(z.meta_words() * 4) +
          DevBuf::alloc_size(z.order_words() * 4);
 }
 template <class F>
-size_t msm_accum_bytes(const MsmShape& sh, uint32_t n) {
-  const MsmSizes z(sh, n);
+size_t msm_accum_bytes(const MsmShape& sh, uint32_t n, uint32_t K = 1) {
+  const MsmSizes z(sh, n, K);
   const size_t x = sizeof(Xyzz<F>);
   return DevBuf::alloc_size(z.max_s0 * x) + DevBuf::alloc_size(z.max_s1 * x) + DevBuf::alloc_size(z.max_s2 * x) +
-         DevBuf::alloc_size((size_t)z.nb1 * x) + DevBuf::alloc_size(MsmReduce<F>(sh).red_elems * x) + DevBuf::alloc_size(x);
+         DevBuf::alloc_size((size_t)z.nb1 * x) + DevBuf::alloc_size(MsmReduce<F>(sh, K).red_elems * x) +
+         DevBuf::alloc_size(K * x);
 }
 
 // Digits, bucket sort and slice order of n scalars into ws; the entries index table slots row * nbases + offset + i.
 // infmask = null keeps the entries of every base: with nbases = n and offset = 0 that is the shared witness sort,
 // which msm_enqueue reads as it is (a table without infinity bases and slots row * n + i) or through msm_view.
+// K > 1: K scalar vectors (proof p's scalar i at (i sstride + p pstride) elements) sorted as one over K k B buckets.
 template <class FrP>
 int msm_sort(MsmWorkspace& ws, const uint32_t* infmask, uint32_t nbases, MsmShape sh, uint32_t offset,
-             const uint32_t* d_scalars, uint32_t sstride, uint32_t n, int mont, cudaStream_t st) {
-  CS_TRY(msm_check_limits(sh, n, nbases));
-  const MsmSizes z(sh, n);
+             const uint32_t* d_scalars, uint32_t sstride, uint32_t n, int mont, cudaStream_t st, uint32_t K = 1,
+             uint32_t pstride = 0) {
+  CS_TRY(msm_check_limits(sh, n, nbases, K));
+  const MsmSizes z(sh, n, K);
   const uint32_t tile = msm_bin_tile(sh, z, n);
-  const uint32_t nblk = n ? ceil_div(n, tile) : 0;
-  const uint32_t NB = sh.nb();
+  const uint32_t nblk_p = n ? ceil_div(n, tile) : 0, nblk = K * nblk_p;
+  const uint32_t NB = sh.nb();  // buckets of one proof
   const dim3 grid(nblk, ceil_div(NB, MSM_BIN_SPAN)), grid_sc(nblk, ceil_div(NB, MSM_SCATTER_SPAN));
   const uint32_t smem = (NB < MSM_BIN_SPAN ? NB : MSM_BIN_SPAN) * 4;
   const uint32_t smem_sc = (NB < MSM_SCATTER_SPAN ? NB : MSM_SCATTER_SPAN) * 4;
@@ -955,21 +1055,21 @@ int msm_sort(MsmWorkspace& ws, const uint32_t* infmask, uint32_t nbases, MsmShap
   CS_TRY(ws.mark(0, st));
   if (nblk)
     CS_LAUNCH_SYNC(k_msm_bin_count<FrP>, grid, MSM_BIN_T, smem, st, d_scalars, sstride, n, mont, sh.c, sh.W, sh.k,
-                   infmask, offset, tile, NB, tab);
+                   infmask, offset, tile, nblk_p, pstride, NB, tab);
   CS_TRY(ws.mark(1, st));
-  CS_LAUNCH(k_msm_bin_scan, ceil_div(NB, 256), 256, 0, st, tab, nblk, NB, q.count);
-  CS_TRY(msm_scan(q, z, NB, st));
+  CS_LAUNCH(k_msm_bin_scan, ceil_div(K * NB, 256), 256, 0, st, tab, nblk_p, NB, K * NB, q.count);
+  CS_TRY(msm_scan(q, z, K * NB, st));
   if (nblk)
     CS_LAUNCH_SYNC(k_msm_bin_scatter<FrP>, grid_sc, MSM_BIN_T, smem_sc, st, d_scalars, sstride, n, mont, sh.c, sh.W, sh.k,
-                   infmask, offset, tile, NB, nbases, tab, q.start, ws.sorted.as<uint32_t>());
+                   infmask, offset, tile, nblk_p, pstride, NB, nbases, tab, q.start, ws.sorted.as<uint32_t>());
   return msm_slice_order(ws, q, z, st);
 }
 
 // This table's entries out of the shared witness sort in src (k_msm_view_*): entries of its infinite bases dropped,
 // the others rewritten to its slots row * nbases + offset + i; then bucket offsets and a slice order of its own.
 static inline int msm_view(MsmWorkspace& ws, const MsmWorkspace& src, const uint32_t* infmask, uint32_t nbases,
-                           MsmShape sh, uint32_t offset, uint32_t n, cudaStream_t st) {
-  const MsmSizes z(sh, n);
+                           MsmShape sh, uint32_t offset, uint32_t n, cudaStream_t st, uint32_t K = 1) {
+  const MsmSizes z(sh, n, K);
   const uint32_t nblk = ceil_div(z.nent, MSM_VIEW_T);
   // dig: keep bitmap | blk_cnt[nblk] | blk_off[nblk + 1]
   CS_TRY(ws.dig.reserve(msm_view_dig_words(z) * 4));
@@ -986,12 +1086,13 @@ static inline int msm_view(MsmWorkspace& ws, const MsmWorkspace& src, const uint
   CS_LAUNCH(k_msm_view_counts, ceil_div(z.nb1, 256), 256, 0, st, s.start, z.nb1, keep, blk_off, q.count);
   CS_LAUNCH(k_msm_view_scatter, nblk, MSM_VIEW_T, 0, st, src_sorted, n, nbases, offset, keep, blk_off,
             ws.sorted.as<uint32_t>());
-  CS_TRY(msm_scan(q, z, sh.nb(), st));
+  CS_TRY(msm_scan(q, z, K * sh.nb(), st));
   return msm_slice_order(ws, q, z, st);
 }
 
-// Enqueue one MSM on `st`.  d_scalars: device, n elements of Fr (8 x u32).  The XYZZ result lands in
-// ws.h_result (pinned) after the stream drains.
+// Enqueue one MSM on `st`.  d_scalars: device, n elements of Fr (8 x u32).  The XYZZ result lands in ws.result and
+// ws.h_result (pinned) after the stream drains.  K > 1: a batch of K MSMs over the same bases (scalar layout as in
+// msm_sort), one sort and accumulation for all; K results.
 // sort_from (optional): a workspace holding a sort of the SAME scalars, enqueued earlier; `st` waits for it.
 //  * view = false: its sorted entries and slice order are used as they are (they index table slots, not points), so
 //    this MSM starts at the accumulation.  Table geometry (nbases, offset, n, window) and infinity pattern must
@@ -1006,32 +1107,35 @@ template <class F, class FrP>
 int msm_enqueue(MsmWorkspace& ws, const Affine<F>* table, const uint32_t* infmask, uint32_t nbases, MsmShape sh,
                 uint32_t offset,
                 const uint32_t* d_scalars, uint32_t sstride, uint32_t n, int mont, cudaStream_t st,
-                MsmWorkspace* sort_from = nullptr, bool view = false, bool table_m260 = false, cudaStream_t st_acc = nullptr) {
-  CS_TRY(msm_check_limits(sh, n, nbases));
-  const MsmSizes z(sh, n);
+                MsmWorkspace* sort_from = nullptr, bool view = false, bool table_m260 = false, cudaStream_t st_acc = nullptr,
+                uint32_t K = 1, uint32_t pstride = 0) {
+  CS_TRY(msm_check_limits(sh, n, nbases, K));
+  const MsmSizes z(sh, n, K);
   const uint32_t nb1 = z.nb1, S = z.S;
   const size_t max_s0 = z.max_s0, max_s1 = z.max_s1, max_s2 = z.max_s2;
   CS_TRY(ws.part0.reserve(max_s0 * sizeof(Xyzz<F>)));
   CS_TRY(ws.part1.reserve(max_s1 * sizeof(Xyzz<F>)));
   CS_TRY(ws.part2.reserve(max_s2 * sizeof(Xyzz<F>)));
   CS_TRY(ws.bucket.reserve((size_t)nb1 * sizeof(Xyzz<F>)));
-  const MsmReduce<F> rd(sh);
-  const uint32_t L = rd.L, nseg = rd.nseg, fs_threads = rd.fs_threads, fs_blocks = rd.fs_blocks;
+  const MsmReduce<F> rd(sh, K);
+  const uint32_t L = rd.L, nseg = rd.nseg, fs_threads = rd.fs_threads, fs_blocks = rd.fs_blocks, G = rd.ngroups;
   CS_TRY(ws.red.reserve(rd.red_elems * sizeof(Xyzz<F>)));
-  CS_TRY(ws.result.reserve(sizeof(Xyzz<F>)));
-  if (ws.h_result_cap < sizeof(Xyzz<F>)) {
+  CS_TRY(ws.result.reserve(K * sizeof(Xyzz<F>)));
+  if (ws.h_result_cap < K * sizeof(Xyzz<F>)) {
     if (ws.h_result) cudaFreeHost(ws.h_result);
-    CS_CUDA(cudaMallocHost(&ws.h_result, sizeof(Xyzz<F>)));
-    ws.h_result_cap = sizeof(Xyzz<F>);
+    ws.h_result = nullptr;
+    ws.h_result_cap = 0;
+    CS_CUDA(cudaMallocHost(&ws.h_result, K * sizeof(Xyzz<F>)));
+    ws.h_result_cap = K * sizeof(Xyzz<F>);
   }
   if (sort_from) {
     if (!sort_from->sorted_once) return fail(-1, "msm: the workspace to share a sort with has not been enqueued");
     CS_TRY(ws.mark(0, st));
     CS_CUDA(cudaStreamWaitEvent(st, sort_from->sorted_ev, 0));
     CS_TRY(ws.mark(1, st));
-    if (view) CS_TRY(msm_view(ws, *sort_from, infmask, nbases, sh, offset, n, st));
+    if (view) CS_TRY(msm_view(ws, *sort_from, infmask, nbases, sh, offset, n, st, K));
   } else {
-    CS_TRY(msm_sort<FrP>(ws, infmask, nbases, sh, offset, d_scalars, sstride, n, mont, st));
+    CS_TRY(msm_sort<FrP>(ws, infmask, nbases, sh, offset, d_scalars, sstride, n, mont, st, K, pstride));
   }
   MsmWorkspace& so = sort_from && !view ? *sort_from : ws;  // owner of the sorted entries
   const MsmSortBufs q(so, z);
@@ -1084,23 +1188,24 @@ int msm_enqueue(MsmWorkspace& ws, const Affine<F>* table, const uint32_t* infmas
   CS_LAUNCH(k_msm_accum2<F>, ceil_div(nb1, 128), 128, 0, st, ws.part2.as<Xyzz<F>>(), sstart2, nb1,
             ws.bucket.as<Xyzz<F>>());
   CS_TRY(ws.mark(4, st));
-  CS_LAUNCH(k_msm_reduce_seg<F>, ceil_div(nseg, 128), 128, 0, st, ws.bucket.as<Xyzz<F>>(), sh.nb(), sh.B, L,
+  CS_LAUNCH(k_msm_reduce_seg<F>, ceil_div(nseg, 128), 128, 0, st, ws.bucket.as<Xyzz<F>>(), K * sh.nb(), sh.B, L,
             ws.red.as<Xyzz<F>>());
-  // one sum per bucket group: the MSM result itself when k = 1, else the group sums that k_msm_combine_groups weights
-  Xyzz<F>* gsum = sh.k > 1 ? ws.red.as<Xyzz<F>>() + nseg + (size_t)sh.k * fs_blocks : ws.result.as<Xyzz<F>>();
+  // one sum per bucket group: the MSM results themselves when k = 1, else the group sums that k_msm_combine_groups weights
+  Xyzz<F>* gsum = sh.k > 1 ? ws.red.as<Xyzz<F>>() + nseg + (size_t)G * fs_blocks : ws.result.as<Xyzz<F>>();
   if (fs_blocks > 1) {
     Xyzz<F>* stage = ws.red.as<Xyzz<F>>() + nseg;
-    CS_LAUNCH_SYNC(k_msm_final_sum<F>, dim3(fs_blocks, sh.k), fs_threads, fs_threads * sizeof(Xyzz<F>), st,
+    CS_LAUNCH_SYNC(k_msm_final_sum<F>, dim3(fs_blocks, G), fs_threads, fs_threads * sizeof(Xyzz<F>), st,
                    ws.red.as<Xyzz<F>>(), rd.nseg_g, stage);
-    CS_LAUNCH_SYNC(k_msm_final_sum<F>, dim3(1, sh.k), fs_threads, fs_threads * sizeof(Xyzz<F>), st, stage, fs_blocks, gsum);
+    CS_LAUNCH_SYNC(k_msm_final_sum<F>, dim3(1, G), fs_threads, fs_threads * sizeof(Xyzz<F>), st, stage, fs_blocks, gsum);
   } else {
-    CS_LAUNCH_SYNC(k_msm_final_sum<F>, dim3(1, sh.k), fs_threads, fs_threads * sizeof(Xyzz<F>), st, ws.red.as<Xyzz<F>>(),
+    CS_LAUNCH_SYNC(k_msm_final_sum<F>, dim3(1, G), fs_threads, fs_threads * sizeof(Xyzz<F>), st, ws.red.as<Xyzz<F>>(),
                    rd.nseg_g, gsum);
   }
-  if (sh.k > 1)
-    CS_LAUNCH(k_msm_combine_groups<F>, 1, 1, 0, st, gsum, sh.k, sh.c, ws.result.as<Xyzz<F>>());
+  // one launch per MSM of a batch: a batch index in the kernel makes its G2 instantiations spill more
+  for (uint32_t p = 0; sh.k > 1 && p < K; p++)
+    CS_LAUNCH(k_msm_combine_groups<F>, 1, 1, 0, st, gsum + (size_t)p * sh.k, sh.k, sh.c, ws.result.as<Xyzz<F>>() + p);
   CS_TRY(ws.mark(5, st));
-  CS_CUDA(cudaMemcpyAsync(ws.h_result, ws.result.p, sizeof(Xyzz<F>), cudaMemcpyDeviceToHost, st));
+  CS_CUDA(cudaMemcpyAsync(ws.h_result, ws.result.p, K * sizeof(Xyzz<F>), cudaMemcpyDeviceToHost, st));
   CS_CUDA(cudaGetLastError());
   return 0;
 }

@@ -20,6 +20,17 @@
 namespace cs {
 
 constexpr unsigned NTT_MAX_K = 10;
+// dynamic shared memory of a pass (ntt_smem_optin): the tile's rows x batch x 32 B, plus rows x 32 B of staged twiddles
+constexpr size_t NTT_SMEM_TWS = 96u << 10, NTT_SMEM_PLAIN = 64u << 10;
+
+// Stages per pass: NTT_MAX_K, or fewer when `batch` columns of 2^k rows would not fit the pass's shared memory (a
+// batch of proofs' vectors, interleaved); 0 = not even two rows fit.  batch <= 2 always gets NTT_MAX_K.
+static inline uint32_t ntt_max_stages(uint32_t batch, bool tws) {
+  const size_t row = ((size_t)batch + (tws ? 1 : 0)) * 32, cap = tws ? NTT_SMEM_TWS : NTT_SMEM_PLAIN;
+  uint32_t k = NTT_MAX_K;
+  while (k && ((size_t)1 << k) * row > cap) k--;
+  return k;
+}
 
 template <class FrP>
 CS_D Fp<FrP> ld_fr(const uint32_t* p) {
@@ -196,8 +207,14 @@ int ntt_enqueue(uint32_t* d_data, const uint32_t* d_tw, uint32_t logn, uint32_t 
     if (d_post || d_scale) return fail(-3, "ntt: size-1 transform with scaling is not supported on device");
     return 0;
   }
-  // split logn into passes of <= NTT_MAX_K stages
-  uint32_t npass = (logn + NTT_MAX_K - 1) / NTT_MAX_K;
+  static int tws_env = -1, thr_env = -1;  // tuning hooks
+  if (tws_env < 0) { const char* e = getenv("CS_NTT_TWS"); tws_env = e ? atoi(e) : 1; }
+  if (thr_env < 0) { const char* e = getenv("CS_NTT_THREADS"); thr_env = e ? atoi(e) : 512; }
+  const bool tws = tws_env != 0;
+  // split logn into passes of <= kmax stages
+  const uint32_t kmax = ntt_max_stages(batch, tws);
+  if (!kmax) return fail(-3, "ntt: %u interleaved columns do not fit a pass's shared memory", batch);
+  uint32_t npass = (logn + kmax - 1) / kmax;
   uint32_t base = logn / npass, extra = logn % npass;
   uint32_t done = 0;
   for (uint32_t p = 0; p < npass; p++) {
@@ -206,10 +223,6 @@ int ntt_enqueue(uint32_t* d_data, const uint32_t* d_tw, uint32_t logn, uint32_t 
     uint32_t log_stride = dit ? done : (logn - done - k);
     bool last = (p + 1 == npass);
     uint32_t rows = 1u << k;
-    static int tws_env = -1, thr_env = -1;  // tuning hooks
-    if (tws_env < 0) { const char* e = getenv("CS_NTT_TWS"); tws_env = e ? atoi(e) : 1; }
-    if (thr_env < 0) { const char* e = getenv("CS_NTT_THREADS"); thr_env = e ? atoi(e) : 512; }
-    const bool tws = tws_env != 0;
     uint32_t threads = (rows / 2) * batch;
     if (threads > (uint32_t)thr_env) threads = thr_env;
     if (threads < 32) threads = 32;

@@ -234,14 +234,19 @@ CS_GLOBAL void k_poly_eval(const uint32_t* __restrict__ coeffs, size_t n, uint32
 //             party 2; plain: 0)   -- arithmetic.rs:52-58
 //   Rows [nrows, nrows + n_pubrows) get the promoted public inputs (reduction.rs:111-113) when
 //   n_pubrows > 0; rows beyond that up to `domain` are zero-filled (reduction.rs:208).
+//   grid.y = proofs of a batch: proof p reads pub + p n_pub and wit + p wpstride elements and writes `batch` columns
+//   from column p batch of out's ocols-column rows (ocols = batch for one proof).
 template <class FrP>
 CS_GLOBAL void k_spmv(const uint32_t* __restrict__ row_ptr, const uint32_t* __restrict__ col,
                       const uint32_t* __restrict__ coeff, const uint32_t* __restrict__ pub, uint32_t n_pub,
                       const uint32_t* __restrict__ wit, uint32_t batch, uint32_t wstride, int pub_comp, uint32_t nrows,
-                      uint32_t n_pubrows, uint32_t domain, uint32_t* __restrict__ out) {
+                      uint32_t n_pubrows, uint32_t domain, uint32_t wpstride, uint32_t ocols, uint32_t* __restrict__ out) {
   constexpr int NW = FrP::N;
   uint32_t r = blockIdx.x * blockDim.x + threadIdx.x;
   if (r >= domain) return;
+  pub += (size_t)blockIdx.y * n_pub * NW;
+  wit += (size_t)blockIdx.y * wpstride * NW;
+  out += ((size_t)r * ocols + (size_t)blockIdx.y * batch) * NW;
   Fp<FrP> acc[2];
   acc[0] = Fp<FrP>::zero();
   acc[1] = Fp<FrP>::zero();
@@ -269,8 +274,8 @@ CS_GLOBAL void k_spmv(const uint32_t* __restrict__ row_ptr, const uint32_t* __re
       if (pub_comp == 0) acc[0] = v; else acc[1] = v;
     }
   }
-  st_fr<FrP>(out + (size_t)r * batch * NW, acc[0]);
-  if (batch == 2) st_fr<FrP>(out + ((size_t)r * batch + 1) * NW, acc[1]);
+  st_fr<FrP>(out, acc[0]);
+  if (batch == 2) st_fr<FrP>(out + NW, acc[1]);
 }
 
 }  // namespace cs

@@ -6,12 +6,17 @@ Groth16::plain_prove with fresh (r, s) or Plonk::plain_prove with fresh blinders
 the zkey), proof written in snarkjs' JSON layout (decimal strings, the layout of
 test_vectors/{Groth16,Plonk}/bn254/multiplier2/circom.proof) plus public.json.
 
+`python -m co_snarks_b200.prove --zkey circuit.zkey --wtns w0.wtns w1.wtns ... --out proof.json` proves several
+witnesses of one Groth16 circuit in one batch (cs_groth16_prove_plain_batch) and writes proof_<i>.json (and, with
+--public-out public.json, public_<i>.json) for witness i.
+
 `python -m co_snarks_b200.prove --zkey circuit.zkey --rep3-shares s.0 s.1 s.2 --out proof.json` is
 `generate-proof groth16 --protocol REP3` for the three parties of one box, from their share files.
 """
 import struct
 import argparse
 import json
+import os
 import secrets
 import time
 
@@ -143,10 +148,42 @@ def prove_rep3_from_share_files(args):
         c.close()
 
 
+def _numbered(path, i):
+    stem, ext = os.path.splitext(path)
+    return "%s_%d%s" % (stem, i, ext)
+
+
+def prove_groth16_batch(args):
+    """One cs_groth16_prove_plain_batch call over the witnesses of args.wtns, fresh (r, s) per proof."""
+    ctx = B.Context(args.device, lib_path=args.lib)
+    t0 = time.time()
+    pk = B.Groth16Key.from_zkey(ctx, args.zkey)
+    cv = pk.curve
+    wits = [B.read_wtns(ctx.lib, w, cv) for w in args.wtns]
+    if any(w.shape != wits[0].shape for w in wits):
+        raise SystemExit("the witness files differ in length")
+    wit = np.stack(wits)
+    t1 = time.time()
+    K = len(wits)
+    rs = _rand_fr(cv, 2 * K)
+    A, Bp, C = pk.prove_plain_batch(wit[:, :pk.ni], wit[:, pk.ni:], rs[:K], rs[K:])
+    t2 = time.time()
+    for i in range(K):
+        with open(_numbered(args.out, i), "w") as f:
+            json.dump(proof_json(ctx.lib, A[i], Bp[i], C[i], cv), f)
+        if args.public_out:
+            with open(_numbered(args.public_out, i), "w") as f:
+                json.dump([str(x) for x in _canon(ctx.lib, wit[i, 1:pk.ni], "fr", cv)], f)
+    print("key+witness load %.1f ms, Generate %d proofs took %.1f ms (one batch)" % ((t1 - t0) * 1e3, K, (t2 - t1) * 1e3))
+    pk.free()
+    ctx.close()
+
+
 def main(argv=None):
     ap = argparse.ArgumentParser(description=__doc__.split("\n")[0])
     ap.add_argument("--zkey", required=True)
-    ap.add_argument("--wtns", default=None)
+    ap.add_argument("--wtns", nargs="+", default=None,
+                    help="witness file; several (Groth16): one batch, proof_<i>.json per witness")
     ap.add_argument("--rep3-shares", nargs=3, default=None, metavar=("PARTY0", "PARTY1", "PARTY2"),
                     help="Groth16, 3-party Rep3: the three parties' share files (co-circom split-witness output) instead of --wtns")
     ap.add_argument("--out", default="proof.json")
@@ -160,6 +197,11 @@ def main(argv=None):
         return prove_rep3_from_share_files(args)
     if not args.wtns:
         raise SystemExit("give --wtns (plain prover) or --rep3-shares")
+    if len(args.wtns) > 1:
+        if zkey_protocol(args.zkey) != 1:
+            raise SystemExit("several --wtns: Groth16 keys only")
+        return prove_groth16_batch(args)
+    args.wtns = args.wtns[0]
     ctx = B.Context(args.device, lib_path=args.lib)
     t0 = time.time()
     if zkey_protocol(args.zkey) == 2:

@@ -93,7 +93,8 @@ int cs_bases_info(const cs_bases* bases, unsigned* window_bits, unsigned* window
                   size_t* device_bytes);
 /* Cap on the device bytes a base set or key created on this context may take (its tables and, for a
  * Groth16 key, the scratch its proofs reserve); 0 = automatic: what the device has free.  For callers
- * that keep several keys on one GPU (e.g. three Rep3 parties), which the library cannot see coming. */
+ * that keep several keys on one GPU (e.g. three Rep3 parties), which the library cannot see coming.
+ * cs_groth16_prove_plain_batch sizes its sub-batches by the same budget. */
 int cs_ctx_set_table_budget(cs_ctx* ctx, size_t bytes);
 int cs_msm(cs_ctx* ctx, const cs_bases* bases, size_t offset, const uint64_t* h_scalars, size_t n,
            int scalars_montgomery, uint64_t* h_out_affine_mont, int* out_is_infinity);
@@ -252,6 +253,24 @@ int cs_groth16_prove_plain(cs_ctx* ctx, cs_groth16_pk* pk, const uint64_t* h_pub
 int cs_groth16_prove_plain_device(cs_ctx* ctx, cs_groth16_pk* pk, const uint64_t* h_public_inputs,
                                   const uint64_t* d_witness, const uint64_t* h_r_mont, const uint64_t* h_s_mont,
                                   uint64_t* out_a, uint64_t* out_b, uint64_t* out_c);
+
+/* A batch of plain proofs of one circuit (plain driver only: there is no Rep3 or Shamir batch; a Rep3
+ * party proves one witness per cs_groth16_rep3_prove call): Groth16::prove (groth16.rs:484-490, CoGroth16::prove with the
+ * plain driver) applied to num_proofs witnesses, proof j with (r[j], s[j]).  Proof j is byte for byte
+ * what cs_groth16_prove_plain returns for public_inputs[j], witness[j], r[j], s[j].
+ *   h_public_inputs: [num_proofs][num_public] incl. the leading 1; witnesses [num_proofs][num_witness],
+ *   on the host (h_witness) or in device memory (d_witness) -- exactly one of the two unless the key
+ *   has no witness.  This is the layout BatchedSharedWitness::unbatch (co-circom-types/src/lib.rs:221-264)
+ *   yields, one witness after the other.  r, s: [num_proofs] Fr (Montgomery).
+ *   Outputs: A [num_proofs] (G1), B [num_proofs] (G2), C [num_proofs] (G1), affine Montgomery.
+ * The batch shares one sort and one accumulation per MSM and does every proof's single-point work on
+ * the device.  It runs in sub-batches sized from the bucket-sort limits and the device memory free at
+ * the call (capped by cs_ctx_set_table_budget); their scratch stays with the key and the context.
+ * num_public / num_witness must match the key (CS_ERR_ARG otherwise). */
+int cs_groth16_prove_plain_batch(cs_ctx* ctx, cs_groth16_pk* pk, size_t num_proofs, const uint64_t* h_public_inputs,
+                                 size_t num_public, const uint64_t* h_witness, const uint64_t* d_witness,
+                                 size_t num_witness, const uint64_t* h_r_mont, const uint64_t* h_s_mont,
+                                 uint64_t* out_a, uint64_t* out_b, uint64_t* out_c);
 
 /* One party's LOCAL part of Rep3CoGroth16::prove up to the first network round
  * (groth16.rs:151-163 + the rayon_join5 block :227-294): witness map, then the five MSMs.

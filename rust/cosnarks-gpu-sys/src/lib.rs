@@ -89,6 +89,10 @@ extern "C" {
     pub fn cs_groth16_prove_plain(ctx: *mut cs_ctx, pk: *mut cs_groth16_pk, public_inputs: *const u64,
                                   witness: *const u64, r: *const u64, s: *const u64, out_a: *mut u64,
                                   out_b: *mut u64, out_c: *mut u64) -> c_int;
+    pub fn cs_groth16_prove_plain_batch(ctx: *mut cs_ctx, pk: *mut cs_groth16_pk, num_proofs: usize,
+                                        public_inputs: *const u64, num_public: usize, h_witness: *const u64,
+                                        d_witness: *const u64, num_witness: usize, r: *const u64, s: *const u64,
+                                        out_a: *mut u64, out_b: *mut u64, out_c: *mut u64) -> c_int;
     // --- transport + Rep3 / Shamir parties inside the library
     pub fn cs_net_from_callbacks(id: c_int, n_parties: c_int, cb: *const cs_net_callbacks, out: *mut *mut cs_net) -> c_int;
     pub fn cs_net_free(net: *mut cs_net);
